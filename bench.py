@@ -2,6 +2,7 @@
 """bench.py — BASELINE.json's metric: GB/s scanned over an HBM-resident synthetic corpus.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--gib G] [--workload NAME] [--no-side]
+                    [--dump-outputs DIR]
 
 Headline (value / roofline / e2e) = BASELINE configs[1]: 8-byte literal over 10 GiB of HBM-resident synthetic ASCII per
 GPU, count + all offsets.  For N>1 (launched by torchrun, one rank per GPU) each rank holds its own 10 GiB shard
@@ -10,12 +11,17 @@ GPU, count + all offsets.  For N>1 (launched by torchrun, one rank per GPU) each
 
 The same JSON line carries a `workloads` object with BASELINE configs[2], [3] and [4] at their stated TOTAL sizes,
 sharded over the N GPUs the run was launched with (strong scaling): -i 4-byte literal on 50 GiB, 1000 patterns on
-20 GiB (20 / 10 / 5 / 2.5 GiB per GPU at N = 1 / 2 / 4 / 8) and -w 16-byte literal on 100 GiB.
+20 GiB (20 / 10 / 5 / 2.5 GiB per GPU at N = 1 / 2 / 4 / 8) and -w 16-byte literal on 40 GiB (every total fits one
+80 GB H100 at N = 1).
 
 A step = one pass of the hot path over the resident shard: filter+verify kernel, the one-CTA finish kernel (count +
 sorted list, one synchronisation), policy replay into krep's match_result_t (N>1: + export, gather, key merge; rank 0
-does its host work for step i while step i+1 scans).  Inputs are >= 2.5 GiB >> 126 MB L2, so nothing survives in L2
+does its host work for step i while step i+1 scans).  Inputs are >= 2.5 GiB >> 50 MB L2, so nothing survives in L2
 between steps.  One JSON line on stdout (rank 0).
+
+--dump-outputs DIR writes what the caller of the timed path received in the last timed step of the headline workload
+(rank 0): DIR/matches.npy (the count) and DIR/positions.npy (the match_result_t (start, end) offsets), float64.  Inputs
+depend only on the arguments, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -61,7 +67,7 @@ WORKLOADS = {
 }
 SEED, PLANT_SEED = 0x5EED0001, 0x5EED0002
 # BASELINE configs[2..4]: (workload, TOTAL GiB over all GPUs) — strong scaling over the N the run is launched with
-SIDE_WORKLOADS = [("icase4", 50.0), ("multi1000", 20.0), ("word16", 100.0)]
+SIDE_WORKLOADS = [("icase4", 50.0), ("multi1000", 20.0), ("word16", 40.0)]
 # at N = 1 only: hit-density sweep on 10 GiB
 DENSITY_WORKLOADS = [("the_1k", 10.0), ("the_64", 10.0), ("the_1k_c", 10.0), ("the_64_c", 10.0), ("multi1000_5to12", 10.0)]
 
@@ -71,7 +77,7 @@ def peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM, HBM3 3.35 TB/s; not measured)"
 
 
 def multi_patterns(n, needle, lens=(6, 12)):
@@ -85,7 +91,7 @@ def multi_patterns(n, needle, lens=(6, 12)):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons (B200_PROFILING.md).  The sampler runs from before the warm-up
+    """nvidia-smi clocks / throttle reasons.  The sampler runs from before the warm-up
     (nvidia-smi takes ~100 ms to produce its first line) and only samples whose timestamp falls inside the
     timed region are reported; if the region was too short to contain one, the nearest samples are used."""
 
@@ -497,7 +503,7 @@ class Runner:
                     "kernel_ms": k, "kernel_ms_per_rank": [k], "ms_per_step_per_rank": [step_ms], "exchange_ms": 0.0,
                     "exchange_ms_per_rank": [0.0], "rank0_host_ms_per_step": 0.0,
                     "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                                 "kernel_ms": k, "algorithmic_bytes_per_launch": total_bytes, "peak_source": peak_src, "traffic": None},
+                                 "kernel_ms": k, "algorithmic_bytes_per_launch": total_bytes, "peak_source": peak_src},
                     "gpu_launches": int(L.krep_b200_launch_count())}
 
         def process(slot):
@@ -623,8 +629,7 @@ class Runner:
                 "exchange_ms": x_max, "exchange_ms_per_rank": x_all, "rank0_host_ms_per_step": state["host_ms"] / max(steps, 1),
                 "steps_overlapped": overlapped,
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "kernel_ms": k_max, "algorithmic_bytes_per_launch": int(per_gpu), "peak_source": peak_src,
-                             "traffic": measured_traffic(name, per_gpu)},
+                             "kernel_ms": k_max, "algorithmic_bytes_per_launch": int(per_gpu), "peak_source": peak_src},
                 "gpu_launches": launches,
             }
         self._last = dict(plan=plan, params=params, res=res, pats=pats, algo=algo, total=int(state["total"]),
@@ -717,17 +722,28 @@ class Runner:
         return out
 
 
-def measured_traffic(name, per_gpu_bytes):
-    """DRAM bytes per launch from the committed ncu --set full capture of this workload's kernel (profiles/), scaled to
-    this run's shard size; None when no capture of the current kernels is on file."""
-    tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    try:
-        tr = json.load(open(tpath)).get(name)
-        if tr:
-            return tr["dram_bytes_per_launch"] * (per_gpu_bytes / tr["corpus_bytes"])
-    except Exception:  # noqa: BLE001
-        pass
-    return None
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, last):
+    """The headline's last timed step as its caller received it: the count krep reports and the match_result_t
+    offsets as (start, end) rows, float64 (exact below 2^53).  A list too long for DUMP_BYTES is reduced to a fixed,
+    seeded sample of rows; their row numbers go to positions_rows.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    res = last["res"].contents
+    n = int(res.count)
+    np.save(os.path.join(out_dir, "matches.npy"), np.array([last["total"]], dtype=np.float64))
+    pos = np.zeros((0, 2), dtype=np.float64)
+    if n:
+        raw = np.ctypeslib.as_array(C.cast(res.positions, C.POINTER(C.c_uint64)), shape=(n, 2))
+        cap = (DUMP_BYTES - (1 << 20)) // 24            # 16 B per row + 8 B for its row number
+        if n > cap:
+            rows = np.unique(np.random.default_rng(0x5EED0004).integers(0, n, size=cap))
+            np.save(os.path.join(out_dir, "positions_rows.npy"), rows.astype(np.float64))
+            raw = raw[rows]
+        pos = raw.astype(np.float64)
+    np.save(os.path.join(out_dir, "positions.npy"), pos)
 
 
 def _main(out_stream):
@@ -744,6 +760,7 @@ def _main(out_stream):
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-side", action="store_true", help="skip the BASELINE configs[2..4] side workloads")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline's last-step outputs as .npy files to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     rank = int(os.environ.get("RANK", "0"))
@@ -775,8 +792,12 @@ def _main(out_stream):
     sampler = ClockSampler(R.local_rank)
     if rank == 0:
         sampler.start()
-    head = R.run(args.workload, world * n, args.steps, args.warmup, sampler)     # weak scaling: n owned bytes per GPU
-    clocks = sampler.stop() if rank == 0 else None
+    try:
+        head = R.run(args.workload, world * n, args.steps, args.warmup, sampler)  # weak scaling: n owned bytes per GPU
+    finally:
+        clocks = sampler.stop() if rank == 0 else None                            # never leave nvidia-smi running
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, R._last)
     e2e = None
     if not args.no_e2e:
         e2e = R.e2e(args.workload, world * n, args.e2e_steps)

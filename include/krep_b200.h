@@ -1,4 +1,4 @@
-/* krep_b200.h — C ABI of the B200-native scan engine that drops in behind krep's
+/* krep_b200.h — C ABI of the H100-native scan engine that drops in behind krep's
  * search_func_t boundary.
  *
  * Every entry point below names the reference interface it replaces as
@@ -86,7 +86,7 @@ typedef uint64_t (*search_func_t)(const search_params_t *params,
  * krep_b200_set_devices / KREP_B200_DEVICES (see below), and the resident-shard
  * API runs each shard on the device that owns its memory.  Returns 0, or a
  * negative value after printing "krep: ..." to stderr (the reference's error
- * convention, krep.c:1933).  There is no CPU fallback: without a usable sm_100
+ * convention, krep.c:1933).  There is no CPU fallback: without a usable sm_90
  * device every search entry point prints an error and aborts the call with
  * count 0 and krep_b200_last_error() != 0. */
 int krep_b200_init(int device);

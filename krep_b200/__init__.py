@@ -1,4 +1,4 @@
-"""krep_b200 — B200-native scan engine behind krep's search_func_t boundary.
+"""krep_b200 — H100-native scan engine behind krep's search_func_t boundary.
 
 The product is the C-ABI shared library built from krep_b200/csrc (see include/krep_b200.h);
 this package only holds the build recipe and the ctypes plumbing used by tests and bench.py.

@@ -1,4 +1,4 @@
-"""Build recipe for libkrep_b200.so (the product: CUDA kernels + C ABI), in-tree, sm_100a only."""
+"""Build recipe for libkrep_b200.so (the product: CUDA kernels + C ABI), in-tree, sm_90a only."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libkrep_b200.so")
 SOURCES = ["engine.cu", "scan_literal.cu", "scan_multi.cu", "scan_count.cu", "host_api.cu", "semantics.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fopenmp,-Wall,-Wno-unused-function", "-Xptxas", "-v"]
 
 

@@ -128,8 +128,8 @@ int visible_devices()
     std::lock_guard<std::mutex> lk(mu);
     if (g_visible >= 0) return g_visible;
     // A process in which this library is the FIRST user of CUDA (the krep CLI) hides the GPUs it is not going to use from
-    // the driver before CUDA initialises: cuInit enumerates every visible GPU, which on the 8-GPU bench box costs 6.8 s
-    // against 0.4 s with one device visible (profiles/r2m8_cuinit.txt).  It will use KREP_B200_DEVICES devices (default
+    // the driver before CUDA initialises: cuInit enumerates every visible GPU, which on an 8-GPU box costs seconds
+    // more than with one device visible.  It will use KREP_B200_DEVICES devices (default
     // 1) — the first ones of CUDA_VISIBLE_DEVICES if that is set.  Not done when the host manages devices itself
     // (krep_b200_init / krep_b200_set_devices called first, or KREP_B200_KEEP_VISIBLE set); harmless when something else
     // (torch) has initialised CUDA already — the variable is only read at initialisation.
@@ -194,9 +194,9 @@ static int ctx_create(DevCtx &E, int device)
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0) // sm_90a code loads on compute capability 9.0 only
     {
-        set_error(-1, "device %d (%s, sm_%d%d) is not an sm_100 part; kernels are built for sm_100a only", device,
+        set_error(-1, "device %d (%s, sm_%d%d) is not an sm_90 part; kernels are built for sm_90a only", device,
                   prop.name, prop.major, prop.minor);
         return -1;
     }
@@ -620,8 +620,7 @@ int reset_counter(DevCtx &E, int slot, cudaStream_t stream)
 // 2048-key pieces and counts, for each of its keys, the keys that order before it (16 lanes per key, each taking every
 // 16th list entry; lanes of one slice read the same word — a broadcast); that count is the key's final position.  n^2
 // compares, 10^8 for 10 240 keys, on 320 CTAs x 16 warps — instead of the 105 barrier-separated passes of a one-CTA
-// bitonic network (165 us measured, profiles/r2c_literal8_launches.csv; one thread per key: 86 us, r2e; 8 lanes per key:
-// 51 us, r2f): with ~10^4 keys the quadratic algorithm is the one that uses the machine.
+// bitonic network: with ~10^4 keys the quadratic algorithm is the one that uses the machine.
 // The last CTA to finish zeroes the scan counter and the done-counter for the slot's next scan.
 // ---------------------------------------------------------------------------------------------
 static constexpr int FIN_THREADS = 512, FIN_SLICES = 16, FIN_KEYS = FIN_THREADS / FIN_SLICES, FIN_PIECE = 2048;
@@ -674,9 +673,9 @@ __global__ void __launch_bounds__(FIN_THREADS) k_finish(unsigned long long *coun
     }
 }
 
-// k_finish of the scan whose kernels were just enqueued on `stream`, on the same stream: at ~25 us it is cheaper to run it
-// between two scans than beside one (a CTA that needs registers on an SM the scan's persistent CTAs already fill only
-// gets there when they exit — measured in run r2d: the overlapped version serialised anyway and slowed the scan's tail).
+// k_finish of the scan whose kernels were just enqueued on `stream`, on the same stream: being short, it is cheaper to run
+// it between two scans than beside one (a CTA that needs registers on an SM the scan's persistent CTAs already fill only
+// gets there when they exit, so an overlapped finish serialises anyway and slows the scan's tail).
 int finish_scan(DevCtx &E, int slot, int want_sort, cudaStream_t stream)
 {
     k_finish<<<PACK_KEYS / FIN_KEYS, FIN_THREADS, 0, stream>>>(slot_counter(E, slot), E.d_list[slot], E.key_cap, E.d_pack[slot],
@@ -1044,7 +1043,7 @@ int krep_b200_init(int device)
 void krep_b200_shutdown(void) { engine_shutdown(); }
 int krep_b200_last_error(void) { return t_err; }
 const char *krep_b200_last_error_string(void) { return t_errmsg; }
-const char *krep_b200_version(void) { return "krep_b200 0.2.0 (sm_100a)"; }
+const char *krep_b200_version(void) { return "krep_b200 0.2.0 (sm_90a)"; }
 int krep_b200_device_count(void)
 {
     warm_join();

@@ -1,7 +1,7 @@
 // engine.h — per-device engine contexts and internal entry points shared by engine.cu / host_api.cu.
 //
 // One process can drive several CUDA devices (krep.c:2851-2905 hands chunks to pool threads; here the chunks of one
-// search call go to the visible B200s): every device the library touches gets a DevCtx — two streams, its occurrence
+// search call go to the visible H100s): every device the library touches gets a DevCtx — two streams, its occurrence
 // list, its staging ring — created on first use.  Plans are compiled once on the host and uploaded to a device the
 // first time it runs them (plan_on_device).
 #pragma once

@@ -200,7 +200,7 @@ static int copy_threads()
     if (!nt)
     {
         const char *v = getenv("KREP_B200_COPY_THREADS");
-        nt = v ? atoi(v) : 8; // host threads per device (8 already saturate one PCIe link: 53 GB/s measured; 32+ oversubscribe and halve it) that move the caller's (pageable) text into the pinned staging ring
+        nt = v ? atoi(v) : 8; // host threads per device (8 saturate one PCIe link; many more oversubscribe it) that move the caller's (pageable) text into the pinned staging ring
         nt = std::max(1, std::min(nt, std::max(1, omp_get_num_procs())));
     }
     return nt;
@@ -404,10 +404,9 @@ static std::vector<int> host_devices(size_t n)
     }
     const int prim = primary_device();
     if (prim < 0) return out;
-    // default: ONE device.  Measured (profiles/r2m2_cli_timing.txt, r2m8_cli_timing.txt): from a pageable file mapping a
-    // second GPU adds nothing — the host side (page faults + staging copies of one process) is the limit, 30-45 GB/s — and
-    // every further context costs 0.15-1.3 s of start-up.  KREP_B200_DEVICES=<k> (or krep_b200_set_devices) spreads the
-    // call over k devices, which pays for pinned host text (110 GB/s on 2, 185 GB/s on 8 devices from one NUMA node).
+    // default: ONE device.  From a pageable file mapping a second GPU adds little — the host side (page faults + staging
+    // copies of one process) is the limit — and every further context costs start-up time.  KREP_B200_DEVICES=<k> (or
+    // krep_b200_set_devices) spreads the call over k devices, which pays for pinned host text.
     int want = 1;
     const char *v = getenv("KREP_B200_DEVICES");
     if (v && *v && atoi(v) > 0) want = atoi(v);
@@ -681,8 +680,8 @@ static uint64_t run_search(int entry_algo, const search_params_t *P, const char 
     {
         // the context is still being created on the warm-up thread: meanwhile fault the caller's pages in (a file the
         // host mapped without MAP_POPULATE) with the staging threads, so that the copy loop later runs at link speed
-        // (opt-in: measured on the bench box, faulting pages in the same process while cuInit / context creation run
-        // more than doubles their time — both sides fight over the address-space lock; profiles/r2b_cli_timing.txt)
+        // (opt-in: faulting pages in the same process while cuInit / context creation run slows both down — they
+        // fight over the address-space lock)
         if (n >= (64u << 20) && getenv("KREP_B200_PREFAULT"))
         {
             trace("search: pre-faulting %zu bytes while the context comes up", n);

@@ -63,8 +63,8 @@ __device__ __forceinline__ bool hit_vec(const uint4 &v, uint32_t fold, uint32_t 
 
 // ------------------------------------------------------------------------------------ WINDOW4
 // The 4-byte window at byte offset 4k+r is (lo >> 8r) | (hi << (32-8r)).  A funnel shift would put it on the ALU
-// pipe next to the compares, which is what bounds this kernel (SHF/LOP3/ISETP all issue there at half rate).  The
-// same value is umulhi(lo, 2^(32-8r)) + hi * 2^(32-8r) — an IMAD.HI and an IMAD on the otherwise idle FMA pipe —
+// pipe next to the compares (SHF/LOP3/ISETP all issue there at half rate).  The
+// same value is umulhi(lo, 2^(32-8r)) + hi * 2^(32-8r) — an IMAD.HI and an IMAD on the FMA pipe —
 // so per text word the ALU pipe only sees the case fold (one LOP3, -i only) and the four compares.  The
 // multipliers come from kernel parameters so that the compiler cannot strength-reduce them back into shifts.
 template <bool MASKED>

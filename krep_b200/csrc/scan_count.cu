@@ -202,8 +202,8 @@ __device__ __forceinline__ void unpack_state(uint64_t k, PartState &S)
     S.seen_nl = f & 8u;
 }
 // One copy of the accounting code for the whole kernel.  Inlined four times per tile (plus the hit-mask code) the kernel
-// grew to 5 400 instructions and spent 64 % of its stall cycles waiting for instruction fetch (ncu, run r2f: 0.32 issued
-// warp-instructions per scheduler cycle); the state and both masks fit into three registers, so the call is cheap.
+// grew to 5 400 instructions and stalled mostly on instruction fetch; the state and both masks fit into three
+// registers, so the call is cheap.
 __device__ __noinline__ uint64_t account_call(uint64_t packed, uint32_t hm, uint32_t nm)
 {
     PartState S;

@@ -1,4 +1,4 @@
-// scan_literal.cu — single-literal scan kernels for sm_100a.
+// scan_literal.cu — single-literal scan kernels for sm_90a.
 //
 // Replaces the inner loops of boyer_moore_search (krep.c:1294-1382), kmp_search (krep.c:1663-1763),
 // memchr_search / memchr_short_search (krep.c:3918-4023, 4396-4500) and the simd_* searches
@@ -229,11 +229,12 @@ __device__ __noinline__ unsigned slow_window4(const LitDevParams &p, uint64_t gr
 // Main loads of the window kernel: the sector that holds a warp's "next word" is touched twice (once as lane 31's
 // next-word load, once as the following warp's vector), so these loads keep the default L2 policy instead of
 // evict-first; KREP_B200_W4_CS=1 at build time restores the streaming hint for comparison.
-// Measured on the B200 (profiles/r2c_window4_variants.md, -i 4-byte literal, 10 GiB): the window kernel is bound by its
-// integer pipe, so everything added to its streaming loop costs: every lane loading its own next word (0) 1.798 ms;
-// lane 31 loading + shuffle (2) 1.858 ms; warp-cooperative emission on top of either 2.25-2.27 ms.  Defaults: 0 / 0.
+// On the H100 a second load per lane is what limits the window kernel: with every lane loading its own next word (0) a
+// -i 4-byte scan of 40 GiB runs at 0.69 TB/s, with lane 31 loading + shuffle (2) at 2.63 TB/s (H100 80GB HBM3, 700 W,
+// same counts); how the windows are extracted (IMAD.HI, PRMT or funnel shift) makes no measurable difference once the
+// load is gone.  Warp-cooperative emission lengthens the streaming loop.  Defaults: 2 / 0.
 #ifndef KREP_B200_W4_NX
-#define KREP_B200_W4_NX 0 // how the window kernel gets the word behind a vector: 0 = every lane loads it, 1 / 2 = shuffle
+#define KREP_B200_W4_NX 2 // how the window kernel gets the word behind a vector: 0 = every lane loads it, 1 / 2 = shuffle
 #endif
 #ifndef KREP_B200_W4_WARP_EMIT
 #define KREP_B200_W4_WARP_EMIT 0
@@ -293,9 +294,8 @@ __global__ void __launch_bounds__(256, 4) k_lit_window4(const __grid_constant__ 
         for (int u = 0; u < UNROLL; u++)
             hm |= hit_vec_w<FOLD, MASKED>(v[u], nx[u], fold, mask, k0, c1, c2, c3) ? (1u << u) : 0u;
         // Needles of 1..3 bytes (MASKED) occur often — `the` once per 7 KiB of English-like text, once per 64 B in the density
-        // sweep — so their kernels emit warp-cooperatively (one atomicAdd per warp and vector: 5x faster at one occurrence
-        // per KiB, run r2d); the 4..6-byte kernels keep the per-occurrence path, whose streaming loop is 25 % shorter
-        // (profiles/r2c_window4_variants.md).
+        // sweep — so their kernels emit warp-cooperatively (one atomicAdd per warp and vector); the 4..6-byte kernels
+        // keep the per-occurrence path, whose streaming loop is shorter.
         if constexpr (MASKED || KREP_B200_W4_WARP_EMIT)
         {
             const uint32_t anyhm = __reduce_or_sync(0xffffffffu, hm);
@@ -331,7 +331,7 @@ __global__ void __launch_bounds__(256, 4) k_lit_window4(const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------ launch
-static int g_occ[6] = {0, 0, 0, 0, 0, 0}; // identical on every device of the box (all sm_100)
+static int g_occ[6] = {0, 0, 0, 0, 0, 0}; // identical on every device of the box (all sm_90)
 
 template <typename K>
 static int occupancy(K kernel)

@@ -1,4 +1,4 @@
-// scan_multi.cu — multi-pattern scan for sm_100a; replaces aho_corasick_search's per-byte goto/fail
+// scan_multi.cu — multi-pattern scan for sm_90a; replaces aho_corasick_search's per-byte goto/fail
 // walk (aho_corasick.c:328-437) and ac_trie_build (aho_corasick.c:111-271).
 //
 // The reference chases pointers through 2 KB trie nodes, one dependent load per text byte.  A GPU at

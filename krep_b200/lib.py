@@ -1,7 +1,7 @@
 """ctypes binding of libkrep_b200.so — plumbing for tests and bench.py, not a second implementation.
 
 The library is loaded from krep_b200/libkrep_b200.so (built in-tree by krep_b200/build.py).  Loading
-never falls back to anything else: if the .so is missing this raises, and if no sm_100 device is
+never falls back to anything else: if the .so is missing this raises, and if no sm_90 device is
 usable every search call reports an error through krep_b200_last_error().
 """
 import ctypes as C

@@ -3,7 +3,8 @@ libkrep_b200.so.
 
 Nothing from the reference is committed: krep.c is read where it lies (KREP_REF_DIR, default
 /root/reference), three textual edits are applied in memory (each anchor must occur exactly once), the
-result is written to build/krep_gpu/ (git-ignored) and compiled with gcc against include/krep_b200.h.
+result is compiled with gcc against include/krep_b200.h into oracle/_ref/ (git-ignored, beside the other
+binaries built from the reference sources).
 
   1. #include "krep_b200.h" after krep.c's own includes (krep.h is included first, so the header's
      type restatement is skipped and krep's own search_params_t / match_result_t are used);
@@ -16,7 +17,7 @@ result is written to build/krep_gpu/ (git-ignored) and compiled with gcc against
   4. main calls krep_b200_warmup() right before it starts searching (krep.c:3818), and the file is mapped
      without MAP_POPULATE for literal searches (krep.c:2679): CUDA start-up overlaps the file handling.
 
-The output binary is build/krep_gpu/krep: same CLI, same output code, GPU scan.
+The output binary is oracle/_ref/krep_gpu: same CLI, same output code, GPU scan.
 """
 import os
 import subprocess
@@ -25,7 +26,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 REF_DIR = os.environ.get("KREP_REF_DIR", "/root/reference")
-OUT_DIR = os.path.join(ROOT, "build", "krep_gpu")
+OUT_DIR = os.path.join(ROOT, "oracle", "_ref")
 LIB_DIR = os.path.join(ROOT, "krep_b200")
 
 
@@ -65,7 +66,7 @@ def available():
 
 def build(force=False):
     """-> path of the GPU-backed krep CLI, or None when neither the reference sources nor a prebuilt binary exist."""
-    out = os.path.join(OUT_DIR, "krep")
+    out = os.path.join(OUT_DIR, "krep_gpu")
     if not available():
         return out if os.path.exists(out) else None
     os.makedirs(OUT_DIR, exist_ok=True)

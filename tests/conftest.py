@@ -12,4 +12,4 @@ os.environ.setdefault("KREP_B200_KEEP_VISIBLE", "1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")

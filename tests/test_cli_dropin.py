@@ -58,7 +58,7 @@ def test_gpu_krep_prints_what_stock_krep_prints(tmp_path, size):
     stock = build_oracle.build_ref()[1]
     gpu = build_krep_gpu.build()
     if not stock or not gpu:
-        pytest.skip("stock or GPU-backed krep binary not available (built in the container that has /root/reference)")
+        pytest.skip("stock or GPU-backed krep binary not available (built only where the reference sources are)")
     # the CLI is a one-shot process: let the library hide the GPUs it does not use (conftest keeps them visible for the
     # in-process tests), or every invocation pays cuInit for the whole box
     env_gpu = {k: v for k, v in os.environ.items() if k != "KREP_B200_KEEP_VISIBLE"}

@@ -19,7 +19,7 @@ def checker():
     return ou.reference() or ou.port()
 
 
-@pytest.mark.parametrize("v", _vectors(), ids=lambda v: f'{v["func"]}:{v["pat"][0][:8]}:{v["src"].split()[0]}')
+@pytest.mark.parametrize("v", _vectors(), ids=lambda v: f'{v["func"]}:{v["pat"][0][:8] or "(empty)"}:{v["src"].split()[0]}')
 def test_reference_test_vectors_through_c_abi(v):
     cnt, pos = lib.search(v["func"], params_from(v), text_from(v), with_result=v.get("res", False))
     assert cnt == v["expect"], v["src"]

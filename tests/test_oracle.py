@@ -3,13 +3,16 @@
 1. against the known-answer vectors of the reference's own tests (tests/golden/reference_vectors.json);
 2. against committed fixtures produced by the compiled, unmodified reference
    (tests/golden/ref_fixtures.json, written by tests/golden/make_fixtures.py in the build container);
-3. when oracle/_ref/libkrep_ref.so is present (build container, or travelled to the GPU box):
-   differentially on seeded random inputs over every option combination.
+3. differentially on seeded random inputs over every option combination, against digests of what the compiled,
+   unmodified reference answered on the same inputs (tests/golden/ref_differential.npz, also written by
+   tests/golden/make_fixtures.py).
 """
+import hashlib
 import json
 import os
 import random
 
+import numpy as np
 import pytest
 
 import oracle_util as ou
@@ -42,7 +45,7 @@ def _vectors():
         return json.load(f)["vectors"]
 
 
-@pytest.mark.parametrize("v", _vectors(), ids=lambda v: f'{v["func"]}:{v["pat"][0][:8]}:{v["src"].split()[0]}')
+@pytest.mark.parametrize("v", _vectors(), ids=lambda v: f'{v["func"]}:{v["pat"][0][:8] or "(empty)"}:{v["src"].split()[0]}')
 def test_port_matches_reference_test_vectors(v):
     cnt, pos = ou.port().run(v["func"], params_from(v), text_from(v), with_result=v.get("res", False))
     assert cnt == v["expect"], v["src"]
@@ -89,7 +92,7 @@ def test_port_matches_committed_reference_fixtures():
 
 
 # ---------------------------------------------------------------------------------------------
-# live differential test against the compiled reference
+# differential test against the compiled reference's stored answers
 # ---------------------------------------------------------------------------------------------
 ALPHABETS = [b"ab", b"abc \n", b"aAbB_ 1\n", b"abcdefghij klmnop\nQRS"]
 
@@ -141,43 +144,43 @@ def random_case(rng, func):
     return pats, text, opts, rng.random() < 0.85
 
 
+# func -> (seed, number of random cases); avx512 / neon answers come from the reference's AVX-512 and NEON builds
+DIFFERENTIAL_CASES = {"boyer_moore": (1, 3000), "kmp": (2, 3000), "memchr": (3, 3000), "memchr_short": (4, 3000),
+                      "sse42": (5, 3000), "aho_corasick": (6, 3000), "avx2": (7, 3000), "avx512": (8, 3000),
+                      "neon": (9, 4000)}
+
+
+def answer_digest(answer):
+    """4-byte digest of a checker's (count, [(start, end), ...]) answer."""
+    return int.from_bytes(hashlib.blake2b(repr(answer).encode(), digest_size=4).digest(), "little")
+
+
+def differential_cases(func):
+    seed, n = DIFFERENTIAL_CASES[func]
+    rng = random.Random(seed)
+    return [random_case(rng, func) for _ in range(n)]
+
+
+def _port_vs_stored_reference_answers(func):
+    want = np.load(os.path.join(GOLD, "ref_differential.npz"))[func]
+    cases = differential_cases(func)
+    assert len(want) == len(cases)
+    for it, (pats, text, opts, with_res) in enumerate(cases):
+        a = ou.port().run(func, Params(pats, **opts), text, with_result=with_res)
+        assert answer_digest(a) == want[it], (func, it, pats, text, opts, with_res, a)
+
+
 @pytest.mark.parametrize("func", list(ou.FUNCS))
 def test_port_vs_compiled_reference_differential(func):
-    ref = ou.reference()
-    if ref is None:
-        pytest.skip("compiled reference not available")
-    rng = random.Random(0xC0FFEE ^ hash(func) & 0xFFFF)
-    rng = random.Random({"boyer_moore": 1, "kmp": 2, "memchr": 3, "memchr_short": 4, "sse42": 5, "aho_corasick": 6,
-                         "avx2": 7}[func])
-    for it in range(3000):
-        pats, text, opts, with_res = random_case(rng, func)
-        a = ou.port().run(func, Params(pats, **opts), text, with_result=with_res)
-        b = ref.run(func, Params(pats, **opts), text, with_result=with_res)
-        assert a == b, (func, pats, text, opts, with_res, a, b)
+    _port_vs_stored_reference_answers(func)
 
 
 def test_port_vs_avx512_build_of_the_reference():
     """simd_avx512_search only exists in the reference's AVX-512 build; pin oracle_avx512_search against it."""
-    ref = ou.reference512()
-    if ref is None:
-        pytest.skip("AVX-512 build of the reference not available / CPU without AVX-512BW")
-    rng = random.Random(8)
-    for it in range(3000):
-        pats, text, opts, with_res = random_case(rng, "avx512")
-        a = ou.port().run("avx512", Params(pats, **opts), text, with_result=with_res)
-        b = ref.run("avx512", Params(pats, **opts), text, with_result=with_res)
-        assert a == b, (pats, text, opts, with_res, a, b)
+    _port_vs_stored_reference_answers("avx512")
 
 
 def test_port_vs_neon_build_of_the_reference():
-    """neon_search only exists in the reference's ARM build; its source is compiled here against a scalar arm_neon.h
-    (five intrinsics) and pins oracle_neon_search."""
-    ref = ou.reference_neon()
-    if ref is None:
-        pytest.skip("NEON build of the reference not available")
-    rng = random.Random(9)
-    for it in range(4000):
-        pats, text, opts, with_res = random_case(rng, "neon")
-        a = ou.port().run("neon", Params(pats, **opts), text, with_result=with_res)
-        b = ref.run("neon", Params(pats, **opts), text, with_result=with_res)
-        assert a == b, (pats, text, opts, with_res, a, b)
+    """neon_search only exists in the reference's ARM build; its source was compiled against a scalar arm_neon.h
+    (five intrinsics) to produce the stored answers that pin oracle_neon_search."""
+    _port_vs_stored_reference_answers("neon")
