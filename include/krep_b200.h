@@ -63,7 +63,7 @@ typedef struct search_params
    bool track_positions;    /* !(-c && !-o) */
    bool whole_word;         /* -w   */
 
-   const void *compiled_regex; /* const regex_t* in krep.h; unused on this path */
+   const void *compiled_regex; /* const regex_t* in krep.h; used by krep_b200_regex_search only */
    ac_trie_t *ac_trie;
    size_t max_count; /* SIZE_MAX = unlimited */
 } search_params_t;
@@ -136,17 +136,31 @@ uint64_t krep_b200_simd_avx512_search(const search_params_t *, const char *, siz
 uint64_t krep_b200_aho_corasick_search(const search_params_t *, const char *, size_t, match_result_t *); /* aho_corasick.c:299 */
 /* the ARM build's kernel; never chosen by krep_b200_select_search_algorithm (which stands in for the x86 AVX2 build) */
 uint64_t krep_b200_neon_search(const search_params_t *, const char *, size_t, match_result_t *);          /* krep.c:4506 */
+/* -E: regex_search (krep.c:1389).  The GPU flags every line the regex can match in (a byte automaton built from the
+ * regex string krep compiles, krep.c:2081-2145, read as a C-locale POSIX ERE under REG_NEWLINE); glibc's regexec on
+ * params->compiled_regex (a const regex_t *) then runs on the flagged lines only, clipped to each run of consecutive
+ * flagged lines.  Count, offsets, -w / -c / -m and every glibc detail are regexec's own.  Only for patterns that
+ * krep_b200_select_search_algorithm accepts; any other pattern makes this entry fail (count 0, krep_b200_last_error).
+ * Accepted: literals and escaped punctuation, '.', bracket expressions with ranges, negation and the classes alpha,
+ * digit, alnum, upper, lower, blank, punct, print, graph, xdigit; ^ $ ( ) | * + ? {m} {m,} {m,n} {,n} (counts <= 255);
+ * \w; \b \B \< \> (the filter treats them as empty: a wider answer, never a narrower one).
+ * Refused (the pattern stays with the host's regex_search): back-references, \` \', \s \S \W, [[:space:]],
+ * [[:cntrl:]], collating elements, any character set that holds '\n' or a newline in the pattern, non-ASCII pattern
+ * bytes, unknown escapes, a process running in a multibyte locale (krep itself never calls setlocale), and automata
+ * above 4096 states or 32 KiB of transition table. */
+uint64_t krep_b200_regex_search(const search_params_t *, const char *, size_t, match_result_t *);
 
 /* Many texts, one launch — what search_directory_recursive (krep.c:3310) calling search_file once per small file
- * becomes when the per-call copy and launch latency matters.  `entry` is one of the ten functions above; text i gets
+ * becomes when the per-call copy and launch latency matters.  `entry` is one of the literal and pattern-set functions
+ * above (not krep_b200_regex_search, which is refused with an error); text i gets
  * exactly the count (counts[i]) and positions (results[i], may be NULL, or results == NULL) that
  * entry(params, texts[i], lens[i], results[i]) would have produced.  Returns 0, or a negative error. */
 int krep_b200_search_batch(search_func_t entry, const search_params_t *params, const char *const *texts,
                            const size_t *lens, size_t n_texts, uint64_t *counts, match_result_t *const *results);
 
-/* krep.c:1771 — same decision order (regex excluded: returns NULL for
- * use_regex, the caller keeps its own regex_search), same globals. The
- * returned pointer is one of the eight functions above. */
+/* krep.c:1771 — same decision order, same globals.  For use_regex it returns
+ * krep_b200_regex_search when the pattern's line automaton compiles, and
+ * NULL when it is refused (the caller keeps its own regex_search then). */
 search_func_t krep_b200_select_search_algorithm(const search_params_t *params);
 /* krep.c:1964 */
 const char *krep_b200_get_algorithm_name(search_func_t func);
@@ -185,13 +199,20 @@ enum
    KREP_B200_ALGO_AVX2 = 5,         /* simd_avx2_search    krep.c:4877 */
    KREP_B200_ALGO_AVX512 = 6,       /* simd_avx512_search  krep.c:5108 */
    KREP_B200_ALGO_AC = 7,           /* aho_corasick_search aho_corasick.c:299 */
-   KREP_B200_ALGO_NEON = 8          /* neon_search         krep.c:4506 */
+   KREP_B200_ALGO_NEON = 8,         /* neon_search         krep.c:4506 */
+   KREP_B200_ALGO_REGEX = 9         /* regex_search        krep.c:1389: keys are flagged line starts */
 };
 
 typedef struct krep_b200_plan krep_b200_plan_t; /* compiled pattern set, device-resident */
 
-/* Compile params->pattern (algo != AC) or params->patterns[] (algo == AC)
- * into filter constants / tables on the current device. NULL on error. */
+/* Compile params->pattern (literal algos), params->patterns[] (algo == AC) or the
+ * regex krep compiles from params->patterns[] (algo == REGEX) into filter
+ * constants / tables on the current device. NULL on error (or refused regex).
+ * A REGEX plan's scan emits one key per line the regex may match in,
+ * (global line start << 3); lines longer than about 4 KiB past a thread's
+ * 256-byte segment, or cut by the shard's end, are flagged without a verdict.
+ * Such keys are confirmed only by krep_b200_replay(KREP_B200_ALGO_REGEX, ...)
+ * with the host text; krep_b200_collect / _search_shards refuse regex plans. */
 krep_b200_plan_t *krep_b200_plan_create(const search_params_t *params, int algo);
 void krep_b200_plan_destroy(krep_b200_plan_t *plan);
 /* Which device filter the plan uses (for bench/config reporting). */
@@ -324,6 +345,15 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan, const search_para
 uint64_t krep_b200_replay(int algo, const search_params_t *params, bool only_matching,
                           const uint64_t *keys, uint64_t nkeys,
                           const char *text, size_t text_len, match_result_t *result);
+/* (KREP_B200_ALGO_REGEX: `keys` are flagged line starts of the whole text, `text` / `text_len` the whole host text —
+ * required — and glibc's regexec on params->compiled_regex decides every match, exactly as krep_b200_regex_search.) */
+
+/* Test hook, host only: runs the line automaton that krep_b200_regex_search would use for params over `text` on the
+ * CPU (no long-line bound) and stores the start offsets of the flagged lines in line_starts[0 .. min(result, cap)).
+ * Returns the number of flagged lines, or -1 when the pattern is refused.  *widened (may be NULL) = 1 when the
+ * automaton accepts more than the regex.  No search entry point calls it. */
+int64_t krep_b200_regex_filter_host(const search_params_t *params, const char *text, size_t n, uint64_t *line_starts,
+                                    uint64_t cap, int *widened);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

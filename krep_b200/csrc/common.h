@@ -58,6 +58,38 @@ struct LitDevParams
     uint32_t want_positions;
 };
 
+// -E plans (regex_dfa.cpp): the line automaton of the regex.  Rows are addressed by offset (state * nclasses), and so
+// are the table entries: next_row = trans[row + cls[byte]].  Row 0 is MATCHED (the line is flagged), row nclasses is
+// DEAD (nothing can match in the rest of the line); the '\n' column holds 0 for states that accept at the end of a line.
+//   regex keys : key = global_line_start << LIT_TAG_BITS (tag bits zero), one per flagged line
+static constexpr uint32_t REGEX_TABLE_BYTES = 32768; // transition table budget: shared memory of k_regex_lines
+static constexpr uint32_t REGEX_MAX_STATES = 4096;
+static constexpr uint32_t REGEX_HALO = 4096; // a line may run this far past its thread's segment before it is flagged unverified
+
+struct RegexDfa
+{
+    uint32_t nstates = 0, nclasses = 0, nl_class = 0;
+    uint32_t start = 0; // row of the line-start state
+    uint8_t cls[256];
+    std::vector<uint16_t> trans;
+    bool widened = false; // the automaton accepts more than the regex (word assertions, -i brackets)
+};
+bool regex_source(const search_params_t *P, std::string *out); // the string krep compiles (krep.c:2081-2145)
+int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why); // 0, or -1 = refused (*why)
+void regex_lines_host(const RegexDfa &D, const char *text, size_t n, std::vector<uint64_t> *line_starts);
+
+struct RegexLaunch
+{
+    const uint8_t *text;
+    uint64_t avail_len, own_begin, own_end, global_offset;
+    int32_t prev_byte, next_byte;
+    const uint16_t *trans; // device copy of RegexDfa::trans followed by the 256-byte class map
+    uint32_t ntrans, nclasses, start, nl_class;
+    uint64_t *out;
+    uint64_t cap;
+    unsigned long long *counter;
+};
+
 struct AcDevTables;  // scan_multi.cu: one device's copy of a pattern set's tables
 struct AcHostTables; // scan_multi.cu: the tables as compiled on the host (uploaded to each device on first use)
 
@@ -69,6 +101,7 @@ struct PlanDev
     bool ready = false;
     uint8_t *d_pat_val = nullptr, *d_pat_mask = nullptr; // literal
     AcDevTables *ac = nullptr;                           // pattern set
+    uint16_t *d_regex = nullptr;                         // regex: transition table + class map
 };
 
 struct Plan
@@ -92,6 +125,10 @@ struct Plan
     std::vector<uint32_t> pat_lens;
     uint32_t min_len = 0, max_len = 0;
     AcHostTables *ach = nullptr;
+    // regex (-E)
+    bool is_regex = false;
+    std::string regex;       // the string krep compiled
+    RegexDfa *rx = nullptr;
     std::string filter_name;
     PlanDev dev[MAX_DEV];
     uint64_t magic = 0x6b7265705f623230ull; // "krep_b20"
@@ -141,6 +178,8 @@ struct AcLaunch
 };
 void launch_ac(const Plan *plan, const AcDevTables *T, const AcLaunch &a, int sm_count, cudaStream_t s);
 void count_launch(int n = 1);
+// regex kernel (scan_regex.cu)
+void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s);
 
 // semantics.cpp — reference control flow replayed over the sorted occurrence list
 struct Replay
@@ -155,6 +194,7 @@ struct Replay
 uint64_t replay_literal(int algo, const search_params_t *P, bool only_matching, uint32_t m,
                         const Replay &r, match_result_t *res);
 uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *res);
+uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res); // needs r.text
 bool result_push(match_result_t *r, size_t s, size_t e);
 
 // C-locale helpers shared by host code (krep.c:125-134, krep.h:298-301)

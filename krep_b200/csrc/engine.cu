@@ -373,8 +373,10 @@ void plan_free(Plan *p)
         cudaFree(pd.d_pat_val);
         cudaFree(pd.d_pat_mask);
         if (pd.ac) ac_free_device(pd.ac);
+        cudaFree(pd.d_regex);
     }
     if (p->ach) ac_free_tables(p);
+    delete p->rx;
     p->magic = 0;
     delete p;
 }
@@ -392,6 +394,22 @@ const PlanDev *plan_on_device(const Plan *plan, DevCtx &C)
     {
         pd.ac = ac_upload_tables(plan);
         if (!pd.ac) return nullptr;
+    }
+    else if (plan->is_regex)
+    {
+        // transition table, padded to 16 bytes, then the class map: k_regex_lines copies both to shared memory as vectors
+        const RegexDfa &D = *plan->rx;
+        std::vector<uint16_t> img(((D.trans.size() + 7) & ~(size_t)7) + 128, 0);
+        std::copy(D.trans.begin(), D.trans.end(), img.begin());
+        memcpy(img.data() + img.size() - 128, D.cls, 256);
+        if (cudaMalloc(&pd.d_regex, img.size() * 2) != cudaSuccess ||
+            cudaMemcpy(pd.d_regex, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess)
+        {
+            set_error(-2, "CUDA allocation failed while uploading the regex automaton to device %d", C.device);
+            cudaFree(pd.d_regex);
+            pd = PlanDev();
+            return nullptr;
+        }
     }
     else
     {
@@ -427,10 +445,46 @@ static bool border_free(const std::string &s, bool cs)
     return pi[m - 1] == 0;
 }
 
+// -E: the line automaton of the regex krep compiled from params->patterns.  nullptr and *why when the compiler refuses
+// the pattern (no error is raised: a refused regex simply stays on the host's regex_search).
+Plan *regex_plan_build(const search_params_t *P, std::string *why)
+{
+    std::string re;
+    if (!regex_source(P, &re))
+    {
+        *why = "no pattern";
+        return nullptr;
+    }
+    RegexDfa *D = new RegexDfa();
+    if (regex_compile(re, !P->case_sensitive, D, why) != 0)
+    {
+        delete D;
+        return nullptr;
+    }
+    Plan *pl = new Plan();
+    pl->algo = KREP_B200_ALGO_REGEX;
+    pl->is_regex = true;
+    pl->case_sensitive = P->case_sensitive;
+    pl->whole_word = P->whole_word ? 1 : 0;
+    pl->regex = re;
+    pl->rx = D;
+    pl->filter_name = D->widened ? "regex-lines-widened" : "regex-lines";
+    std::lock_guard<std::mutex> lp(g_plans_mu);
+    g_all_plans.push_back(pl);
+    return pl;
+}
+
 // Maps (reference function, params) to what the device has to enumerate.
 Plan *plan_build(const search_params_t *P, int algo, bool only_matching)
 {
     if (!P) return nullptr;
+    if (algo == KREP_B200_ALGO_REGEX)
+    {
+        std::string why;
+        Plan *pl = regex_plan_build(P, &why);
+        if (!pl) set_error(-3, "this regex is not run on the GPU (%s); use the host's regex_search", why.c_str());
+        return pl;
+    }
     Plan *pl = new Plan();
     pl->algo = algo;
     pl->case_sensitive = P->case_sensitive;
@@ -534,6 +588,27 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
     const PlanDev *pd = plan_on_device(plan, E);
     if (!pd) return -2;
     uint64_t own_end = sh->own_end < sh->avail_len ? sh->own_end : sh->avail_len;
+    if (plan->is_regex)
+    {
+        RegexLaunch a;
+        a.text = (const uint8_t *)sh->d_text;
+        a.avail_len = sh->avail_len;
+        a.own_begin = sh->own_begin;
+        a.own_end = own_end;
+        a.global_offset = sh->global_offset;
+        a.prev_byte = sh->prev_byte;
+        a.next_byte = sh->next_byte;
+        a.trans = pd->d_regex;
+        a.ntrans = (uint32_t)plan->rx->trans.size();
+        a.nclasses = plan->rx->nclasses;
+        a.start = plan->rx->start;
+        a.nl_class = plan->rx->nl_class;
+        a.out = E.d_list[slot];
+        a.cap = want_positions ? E.key_cap : 0;
+        a.counter = slot_counter(E, slot);
+        launch_regex(a, E.sm_count, stream);
+        return 0;
+    }
     if (plan->is_ac)
     {
         // the key packs (global end offset << 24): 40 bits of offset

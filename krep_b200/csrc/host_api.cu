@@ -56,6 +56,7 @@ static std::vector<Plan *> g_plan_cache; // most recent last; plans are device-i
 
 static bool plan_matches(const Plan *pl, const search_params_t *P, int algo, bool only_matching)
 {
+    if (pl->is_regex || algo == KREP_B200_ALGO_REGEX) return false; // regex plans: cached_regex_plan
     if (pl->algo != algo || pl->case_sensitive != P->case_sensitive || pl->count_lines != P->count_lines_mode) return false;
     if (pl->is_ac)
     {
@@ -74,6 +75,16 @@ static bool plan_matches(const Plan *pl, const search_params_t *P, int algo, boo
     return pl->built_only_matching == only_matching;
 }
 
+static void cache_insert(Plan *pl)
+{
+    if (g_plan_cache.size() >= 16)
+    {
+        plan_free(g_plan_cache.front());
+        g_plan_cache.erase(g_plan_cache.begin());
+    }
+    g_plan_cache.push_back(pl);
+}
+
 static Plan *cached_plan(const search_params_t *P, int algo, bool only_matching)
 {
     for (size_t i = 0; i < g_plan_cache.size(); i++)
@@ -85,13 +96,32 @@ static Plan *cached_plan(const search_params_t *P, int algo, bool only_matching)
             return pl;
         }
     Plan *pl = plan_build(P, algo, only_matching);
-    if (!pl) return nullptr;
-    if (g_plan_cache.size() >= 16)
+    if (pl) cache_insert(pl);
+    return pl;
+}
+
+// The regex plan of params (keyed by the regex string krep compiles and the case flag); nullptr and *why when the
+// compiler refuses the pattern.  Host only: no device is touched until the plan runs.
+static Plan *cached_regex_plan(const search_params_t *P, std::string *why)
+{
+    std::string re;
+    if (!regex_source(P, &re))
     {
-        plan_free(g_plan_cache.front());
-        g_plan_cache.erase(g_plan_cache.begin());
+        *why = "no pattern";
+        return nullptr;
     }
-    g_plan_cache.push_back(pl);
+    for (size_t i = 0; i < g_plan_cache.size(); i++)
+    {
+        Plan *pl = g_plan_cache[i];
+        if (pl->is_regex && pl->regex == re && pl->case_sensitive == P->case_sensitive)
+        {
+            g_plan_cache.erase(g_plan_cache.begin() + i);
+            g_plan_cache.push_back(pl);
+            return pl;
+        }
+    }
+    Plan *pl = regex_plan_build(P, why);
+    if (pl) cache_insert(pl);
     return pl;
 }
 
@@ -293,7 +323,8 @@ static int stream_range(RangeJob &J)
     CKH(cudaSetDevice(E.device));
     const Plan *plan = J.plan;
     if (!plan_on_device(plan, E)) return -2;
-    const uint32_t halo = (plan->is_ac ? plan->max_len : plan->m) + 1; // occurrence + the byte after it (-w)
+    // occurrence + the byte after it (-w); regex: how far a line may run past its thread's segment (scan_regex.cu)
+    const uint32_t halo = plan->is_regex ? REGEX_HALO : (plan->is_ac ? plan->max_len : plan->m) + 1;
     const size_t chunk = J.chunk, n = J.n;
     const size_t span = J.end - J.begin;
     const size_t nchunks = (span + chunk - 1) / chunk;
@@ -721,6 +752,42 @@ static uint64_t run_search(int entry_algo, const search_params_t *P, const char 
     return ret;
 }
 
+// -E (regex_search, krep.c:1389): the device flags the lines the regex can match in (k_regex_lines), glibc's regexec
+// on the caller's regex_t confirms them and computes every offset (replay_regex).  The empty text is answered on the
+// host, as the reference does, without a launch.
+static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, match_result_t *res)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    if (!P) return 0;
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
+    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    Replay r{nullptr, 0, text, n, 0};
+    if (n == 0) return replay_regex(P, r, res); // krep.c:1403-1416
+    if (!text) return 0;
+    warm_join();
+    if (visible_devices() == 0)
+    {
+        set_error(-1, "no CUDA device available; this engine has no CPU fallback");
+        return 0;
+    }
+    DeviceGuard guard;
+    std::string why;
+    Plan *plan = cached_regex_plan(P, &why);
+    if (!plan)
+    {
+        set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
+        return 0;
+    }
+    HostScan hs;
+    if (stage_and_scan(plan, text, n, 1, &hs) != 0) return 0;
+    r.keys = hs.keys;
+    r.n = (size_t)hs.nkeys;
+    const uint64_t ret = replay_regex(P, r, res);
+    trace("search: regex confirmed on %llu flagged lines (%llu)", (unsigned long long)hs.nkeys, (unsigned long long)ret);
+    return ret;
+}
+
 // Many texts, one launch (SURVEY §8 f4: small files lose to launch and copy latency one by one).  The texts are packed
 // into one pinned buffer at 16-byte aligned offsets, separated by zero gaps longer than the longest pattern, copied and
 // scanned as ONE shard; the sorted occurrence list is then cut per text — an occurrence belongs to a text only if it
@@ -876,6 +943,10 @@ uint64_t krep_b200_neon_search(const search_params_t *p, const char *t, size_t n
 {
     return run_search(KREP_B200_ALGO_NEON, p, t, n, r);
 }
+uint64_t krep_b200_regex_search(const search_params_t *p, const char *t, size_t n, match_result_t *r)
+{
+    return run_regex(p, t, n, r);
+}
 
 int krep_b200_search_batch(search_func_t entry, const search_params_t *params, const char *const *texts, const size_t *lens,
                            size_t n_texts, uint64_t *counts, match_result_t *const *results)
@@ -890,6 +961,11 @@ int krep_b200_search_batch(search_func_t entry, const search_params_t *params, c
     else if (entry == krep_b200_simd_avx512_search) algo = KREP_B200_ALGO_AVX512;
     else if (entry == krep_b200_aho_corasick_search) algo = KREP_B200_ALGO_AC;
     else if (entry == krep_b200_neon_search) algo = KREP_B200_ALGO_NEON;
+    if (entry == krep_b200_regex_search)
+    {
+        set_error(-3, "krep_b200_search_batch: regex searches are not batched; call krep_b200_regex_search per text");
+        return -3;
+    }
     if (algo < 0)
     {
         set_error(-3, "krep_b200_search_batch: entry must be one of this library's search_func_t entry points");
@@ -928,7 +1004,15 @@ static bool is_repetitive_pattern(const char *pattern, size_t len)
 // krep.c:1771-1870, for the AVX2 build of the reference (SIMD_MAX_PATTERN_LEN 32).
 search_func_t krep_b200_select_search_algorithm(const search_params_t *P)
 {
-    if (!P || P->use_regex) return NULL; // regex stays with the host's regex_search
+    if (!P) return NULL;
+    if (P->use_regex)
+    {
+        // the regex goes to the GPU line filter when its compiler accepts the pattern; a refused one stays with the
+        // host's regex_search
+        std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+        std::string why;
+        return cached_regex_plan(P, &why) ? krep_b200_regex_search : NULL;
+    }
     if (P->num_patterns > 1) return krep_b200_aho_corasick_search;
     if (!g_algo_override.empty() && g_algo_override != "auto")
     {
@@ -955,6 +1039,7 @@ const char *krep_b200_get_algorithm_name(search_func_t f)
     if (f == krep_b200_simd_avx2_search) return "AVX2";
     if (f == krep_b200_simd_avx512_search) return "AVX-512";
     if (f == krep_b200_neon_search) return "NEON";
+    if (f == krep_b200_regex_search) return "Regex (GPU line filter + regexec)";
     return "Unknown";
 }
 
@@ -1047,6 +1132,16 @@ uint64_t krep_b200_replay(int algo, const search_params_t *P, bool only_matching
         set_error(-3, "krep_b200_replay: -c line counting needs the host text");
         return 0;
     }
+    if (algo == KREP_B200_ALGO_REGEX)
+    {
+        clear_error();
+        if (!text && text_len)
+        {
+            set_error(-3, "krep_b200_replay: regex keys are confirmed by regexec on the host text");
+            return 0;
+        }
+        return replay_regex(P, Replay{keys, (size_t)nkeys, text, text_len, 0}, result);
+    }
     Replay r{keys, (size_t)nkeys, text, text_len ? text_len : (SIZE_MAX >> 1), 0};
     if (algo == KREP_B200_ALGO_AC) return replay_ac(P, r, result);
     algo = resolve_algo(P, algo);
@@ -1058,6 +1153,11 @@ uint64_t krep_b200_replay_lines(int algo, const search_params_t *P, bool only_ma
                                 const uint64_t *bounds, size_t text_len, match_result_t *result)
 {
     if (!P) return 0;
+    if (algo == KREP_B200_ALGO_REGEX)
+    {
+        set_error(-3, "krep_b200_replay_lines: regex keys need the host text (krep_b200_replay)");
+        return 0;
+    }
     if (P->count_lines_mode && !bounds && nkeys)
     {
         set_error(-3, "krep_b200_replay_lines: -c needs the line bounds");
@@ -1136,6 +1236,12 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan_, const search_par
     if (!plan || !P || (!shards && n_shards))
     {
         set_error(-3, "krep_b200_search_shards: null argument");
+        return 0;
+    }
+    if (plan->is_regex)
+    {
+        set_error(-3, "krep_b200_search_shards: regex plans need the host text: scan the shards, merge the keys and call "
+                      "krep_b200_replay with KREP_B200_ALGO_REGEX");
         return 0;
     }
     DeviceGuard guard;
@@ -1245,6 +1351,12 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan_, const search_params_t 
     clear_error();
     const Plan *plan = reinterpret_cast<const Plan *>(plan_);
     if (!plan || !P || !dev) return 0;
+    if (plan->is_regex)
+    {
+        set_error(-3, "krep_b200_collect: regex plans need the host text: export the keys and call krep_b200_replay with "
+                      "KREP_B200_ALGO_REGEX");
+        return 0;
+    }
     if (P->count_lines_mode && dev->stored && !dev->d_line_bounds)
     {
         set_error(-3, "krep_b200_collect: -c needs a plan created with count_lines_mode (line bounds are computed by the scan)");
@@ -1303,6 +1415,21 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan_, const search_params_t 
     }
     if (plan->is_ac) return replay_ac(P, r, result);
     return replay_literal(plan->algo, P, plan->built_only_matching, plan->m, r, result);
+}
+
+// ---- test hook: the line filter of a regex plan, run on the host ----
+int64_t krep_b200_regex_filter_host(const search_params_t *P, const char *text, size_t n, uint64_t *line_starts, uint64_t cap,
+                                    int *widened)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl) return -1;
+    std::vector<uint64_t> v;
+    regex_lines_host(*pl->rx, text, text ? n : 0, &v);
+    for (size_t i = 0; i < v.size() && i < cap; i++) line_starts[i] = v[i];
+    if (widened) *widened = pl->rx->widened ? 1 : 0;
+    return (int64_t)v.size();
 }
 
 } // extern "C"

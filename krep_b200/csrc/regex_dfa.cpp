@@ -1,0 +1,643 @@
+// regex_dfa.cpp — the host half of -E searches: rebuilds the regular expression krep compiled (krep.c:2081-2145,
+// 2539-2600), parses it as a glibc POSIX ERE in the C locale and compiles it into a LINE automaton: a DFA that reads
+// one line (the bytes between two '\n') and tells whether the regex can match somewhere in it.
+//
+// The automaton is a filter, not a matcher.  It may say "yes" for a line glibc would not match (its answer is
+// widened wherever modelling glibc exactly would take effort: \b \B \< \> become empty, -i turns every bracket
+// expression into its case closure), never "no" for a line glibc matches.  Positions, leftmost-longest choice, -w, -c
+// and -m all come from glibc's regexec on the caller's own regex_t, run on the flagged lines only (replay_regex).
+// Anything the parser does not know is refused, and a refused pattern stays on the host's regex_search.
+//
+// Under REG_NEWLINE (krep always sets it) no match contains a '\n' as long as no character set of the pattern contains
+// one: '.' and non-matching lists exclude it, but \s, \W, [[:space:]] and [[:cntrl:]] do not — those are refused.
+#include <algorithm>
+#include <bitset>
+#include <climits>
+#include <cstdlib>
+#include <cstring>
+#include <map>
+#include <string>
+#include <vector>
+#include "common.h"
+
+namespace kb {
+
+namespace {
+
+using CharSet = std::bitset<256>;
+
+struct Ast
+{
+    enum Kind { EMPTY, SET, CAT, ALT, REP, BOL, EOL } kind = EMPTY;
+    CharSet set;                 // SET
+    std::vector<int> kids;       // CAT / ALT / REP (one kid)
+    int min = 0, max = 0;        // REP; max < 0 = unbounded
+};
+
+struct Parser
+{
+    const std::string &s;
+    size_t i = 0;
+    bool icase;
+    bool widened = false;
+    std::string why; // non-empty once the pattern is refused
+    std::vector<Ast> nodes;
+
+    Parser(const std::string &src, bool ic) : s(src), icase(ic) {}
+
+    int add(Ast a)
+    {
+        nodes.push_back(std::move(a));
+        return (int)nodes.size() - 1;
+    }
+    int refuse(const char *msg)
+    {
+        if (why.empty()) why = msg;
+        return -1;
+    }
+    int leaf(Ast::Kind k)
+    {
+        Ast a;
+        a.kind = k;
+        return add(a);
+    }
+    int set_node(CharSet cs, bool from_bracket)
+    {
+        if (icase)
+        {
+            CharSet c2 = cs;
+            for (int c = 'A'; c <= 'Z'; c++)
+                if (cs[c] || cs[c + 32]) c2[c] = c2[c + 32] = true;
+            if (from_bracket && c2 != cs) widened = true; // glibc's -i bracket rules are not modelled: take the case closure
+            cs = c2;
+        }
+        if (cs['\n']) return refuse("a character set of the pattern contains the newline");
+        Ast a;
+        a.kind = Ast::SET;
+        a.set = cs;
+        return add(a);
+    }
+
+    int parse_alt()
+    {
+        std::vector<int> br{parse_cat()};
+        while (br.back() >= 0 && i < s.size() && s[i] == '|')
+        {
+            i++;
+            br.push_back(parse_cat());
+        }
+        if (br.back() < 0) return -1;
+        if (br.size() == 1) return br[0];
+        Ast a;
+        a.kind = Ast::ALT;
+        a.kids = br;
+        return add(a);
+    }
+
+    int parse_cat()
+    {
+        std::vector<int> items;
+        while (i < s.size() && s[i] != '|' && s[i] != ')')
+        {
+            int r = parse_repeat();
+            if (r < 0) return -1;
+            items.push_back(r);
+        }
+        if (items.empty()) return leaf(Ast::EMPTY);
+        if (items.size() == 1) return items[0];
+        Ast a;
+        a.kind = Ast::CAT;
+        a.kids = items;
+        return add(a);
+    }
+
+    bool number(int *v)
+    {
+        if (i >= s.size() || s[i] < '0' || s[i] > '9') return false;
+        long x = 0;
+        while (i < s.size() && s[i] >= '0' && s[i] <= '9')
+        {
+            x = x * 10 + (s[i++] - '0');
+            if (x > 255) return false; // larger counts: refused (the expansion would exceed the automaton budget anyway)
+        }
+        *v = (int)x;
+        return true;
+    }
+
+    int parse_repeat()
+    {
+        int atom = parse_atom();
+        while (atom >= 0 && i < s.size())
+        {
+            int mn, mx;
+            const char c = s[i];
+            if (c == '*') mn = 0, mx = -1, i++;
+            else if (c == '+') mn = 1, mx = -1, i++;
+            else if (c == '?') mn = 0, mx = 1, i++;
+            else if (c == '{')
+            {
+                i++;
+                mn = 0;
+                const bool has_min = number(&mn);
+                if (i < s.size() && s[i] == '}')
+                {
+                    if (!has_min) return refuse("empty interval");
+                    mx = mn;
+                }
+                else if (i < s.size() && s[i] == ',')
+                {
+                    i++;
+                    mx = -1;
+                    if (i < s.size() && s[i] != '}' && !number(&mx)) return refuse("interval bound");
+                }
+                else return refuse("interval");
+                if (i >= s.size() || s[i] != '}') return refuse("interval");
+                i++;
+                if (mx >= 0 && mx < mn) return refuse("interval bounds");
+            }
+            else break;
+            Ast a;
+            a.kind = Ast::REP;
+            a.kids = {atom};
+            a.min = mn;
+            a.max = mx;
+            atom = add(a);
+        }
+        return atom;
+    }
+
+    int parse_atom()
+    {
+        const unsigned char c = (unsigned char)s[i];
+        switch (c)
+        {
+        case '(':
+        {
+            i++;
+            int r = parse_alt();
+            if (r < 0) return -1;
+            if (i >= s.size() || s[i] != ')') return refuse("unbalanced parenthesis");
+            i++;
+            return r;
+        }
+        case ')': return refuse("unmatched ')'");
+        case '*': case '+': case '?': case '{': return refuse("repetition without an operand");
+        case '^': i++; return leaf(Ast::BOL);
+        case '$': i++; return leaf(Ast::EOL);
+        case '.':
+        {
+            i++;
+            CharSet cs;
+            cs.set();
+            cs['\n'] = false; // REG_NEWLINE
+            cs[0] = false;    // RE_DOT_NOT_NULL (POSIX syntax)
+            return set_node(cs, false);
+        }
+        case '[': i++; return parse_bracket();
+        case '\\': i++; return parse_escape();
+        default:
+        {
+            i++;
+            if (c == '\n') return refuse("newline in the pattern");
+            if (c >= 0x80) return refuse("non-ASCII byte in the pattern");
+            CharSet cs;
+            cs[c] = true;
+            return set_node(cs, false);
+        }
+        }
+    }
+
+    int parse_escape()
+    {
+        if (i >= s.size()) return refuse("trailing backslash");
+        const unsigned char c = (unsigned char)s[i++];
+        CharSet cs;
+        switch (c)
+        {
+        case 'b': case 'B': case '<': case '>':
+            widened = true; // word assertions: matched by the empty string (a wider answer, see the file comment)
+            return leaf(Ast::EMPTY);
+        case 'w':
+            for (int k = 0; k < 256; k++) cs[k] = is_word_c(k);
+            return set_node(cs, false);
+        case 'W': case 's': case 'S': case '`': case '\'':
+            // \W and \s match '\n' (even under REG_NEWLINE); \S is left out with them; \` \' are buffer anchors
+            return refuse("unsupported escape");
+        default:
+            if (c >= '1' && c <= '9') return refuse("back-reference");
+            if ((c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || (c >= '0' && c <= '9') || c >= 0x80 || c == '\n')
+                return refuse("unknown escape");
+            cs[c] = true; // an escaped punctuation character stands for itself
+            return set_node(cs, false);
+        }
+    }
+
+    bool char_class(const std::string &name, CharSet *cs)
+    {
+        for (int k = 0; k < 128; k++)
+        {
+            bool in;
+            if (name == "alpha") in = is_alpha_c(k);
+            else if (name == "digit") in = k >= '0' && k <= '9';
+            else if (name == "alnum") in = is_alpha_c(k) || (k >= '0' && k <= '9');
+            else if (name == "upper") in = k >= 'A' && k <= 'Z';
+            else if (name == "lower") in = k >= 'a' && k <= 'z';
+            else if (name == "blank") in = k == ' ' || k == '\t';
+            else if (name == "punct") in = k > 32 && k < 127 && !is_alpha_c(k) && !(k >= '0' && k <= '9');
+            else if (name == "print") in = k >= 32 && k < 127;
+            else if (name == "graph") in = k > 32 && k < 127;
+            else if (name == "xdigit") in = (k >= '0' && k <= '9') || (k >= 'a' && k <= 'f') || (k >= 'A' && k <= 'F');
+            else return false; // space / cntrl hold '\n'; anything else is unknown
+            if (in) (*cs)[k] = true;
+        }
+        return true;
+    }
+
+    int parse_bracket()
+    {
+        CharSet cs;
+        bool neg = false;
+        if (i < s.size() && s[i] == '^') neg = true, i++;
+        bool first = true;
+        for (;;)
+        {
+            if (i >= s.size()) return refuse("unterminated bracket expression");
+            unsigned char c = (unsigned char)s[i];
+            if (c == ']' && !first)
+            {
+                i++;
+                break;
+            }
+            first = false;
+            if (c == '[' && i + 1 < s.size() && (s[i + 1] == '.' || s[i + 1] == '=')) return refuse("collating element");
+            if (c == '[' && i + 1 < s.size() && s[i + 1] == ':')
+            {
+                const size_t e = s.find(":]", i + 2);
+                if (e == std::string::npos || !char_class(s.substr(i + 2, e - i - 2), &cs)) return refuse("character class");
+                i = e + 2;
+                if (i < s.size() && s[i] == '-' && i + 1 < s.size() && s[i + 1] != ']') return refuse("range from a class");
+                continue;
+            }
+            if (c >= 0x80) return refuse("non-ASCII byte in the pattern");
+            i++;
+            if (i + 1 < s.size() && s[i] == '-' && s[i + 1] != ']')
+            {
+                const unsigned char d = (unsigned char)s[i + 1];
+                if (d == '[' || d >= 0x80 || d < c) return refuse("range");
+                i += 2;
+                for (int k = c; k <= d; k++) cs[k] = true;
+            }
+            else cs[c] = true;
+        }
+        if (neg)
+        {
+            cs.flip();
+            cs['\n'] = false; // REG_NEWLINE: a non-matching list never matches the newline
+        }
+        return set_node(cs, true);
+    }
+};
+
+// ---- Thompson NFA ------------------------------------------------------------------------------------------------
+struct NState
+{
+    enum Kind { CHAR, SPLIT, BOL, EOL, MATCH } kind;
+    int set = -1;      // CHAR: index into Nfa::sets
+    int out = -1, out1 = -1;
+};
+
+struct Nfa
+{
+    std::vector<NState> st;
+    std::vector<CharSet> sets;
+    bool too_big = false;
+    bool widened = false;
+    static constexpr size_t MAX_STATES = 8192;
+
+    int add(NState::Kind k)
+    {
+        if (st.size() >= MAX_STATES) too_big = true;
+        st.push_back(NState{k});
+        return (int)st.size() - 1;
+    }
+    // Fragment: entry state and the list of dangling exits (state index, which out)
+    struct Frag
+    {
+        int in;
+        std::vector<std::pair<int, int>> outs;
+    };
+    void patch(const Frag &f, int to)
+    {
+        for (auto &o : f.outs) (o.second ? st[o.first].out1 : st[o.first].out) = to;
+    }
+    // in_rep: inside a repeated group, where glibc's anchors do not behave as anchors (it matches "(^a){2}" on "aa"):
+    // ^ and $ there are built as empty (a wider answer)
+    Frag build(const std::vector<Ast> &A, int n, bool in_rep = false)
+    {
+        if (too_big) return Frag{add(NState::SPLIT), {}};
+        const Ast &a = A[n];
+        switch (a.kind)
+        {
+        case Ast::SET:
+        {
+            int s = add(NState::CHAR);
+            st[s].set = (int)sets.size();
+            sets.push_back(a.set);
+            return Frag{s, {{s, 0}}};
+        }
+        case Ast::BOL: case Ast::EOL: case Ast::EMPTY:
+        {
+            if (in_rep && a.kind != Ast::EMPTY) widened = true;
+            const NState::Kind k = in_rep ? NState::SPLIT : a.kind == Ast::BOL ? NState::BOL : a.kind == Ast::EOL ? NState::EOL : NState::SPLIT;
+            int s = add(k);
+            return Frag{s, {{s, 0}}}; // an EMPTY split has out1 = -1: a plain epsilon edge
+        }
+        case Ast::CAT:
+        {
+            Frag f = build(A, a.kids[0], in_rep);
+            for (size_t k = 1; k < a.kids.size(); k++)
+            {
+                Frag g = build(A, a.kids[k], in_rep);
+                patch(f, g.in);
+                f.outs = g.outs;
+            }
+            return f;
+        }
+        case Ast::ALT:
+        {
+            Frag f = build(A, a.kids[0], in_rep);
+            for (size_t k = 1; k < a.kids.size(); k++)
+            {
+                Frag g = build(A, a.kids[k], in_rep);
+                int s = add(NState::SPLIT);
+                st[s].out = f.in;
+                st[s].out1 = g.in;
+                f.in = s;
+                f.outs.insert(f.outs.end(), g.outs.begin(), g.outs.end());
+            }
+            return f;
+        }
+        case Ast::REP:
+        default:
+        {
+            // x{m,n} = x^m (x?)^(n-m);  x{m,} = x^m x*;  each copy is a fresh fragment
+            int entry = add(NState::SPLIT); // epsilon entry (keeps zero-repetition cases uniform)
+            Frag f{entry, {{entry, 0}}};
+            const bool rep = in_rep || a.max != 1 || a.min > 1;
+            for (int k = 0; k < a.min; k++)
+            {
+                Frag g = build(A, a.kids[0], rep);
+                patch(f, g.in);
+                f.outs = g.outs;
+            }
+            if (a.max < 0)
+            {
+                Frag g = build(A, a.kids[0], rep);
+                int s = add(NState::SPLIT);
+                st[s].out = g.in;
+                patch(g, s);
+                patch(f, s);
+                f.outs = {{s, 1}};
+            }
+            else
+            {
+                std::vector<std::pair<int, int>> exits;
+                for (int k = a.min; k < a.max; k++)
+                {
+                    Frag g = build(A, a.kids[0], rep);
+                    int s = add(NState::SPLIT);
+                    st[s].out = g.in;
+                    patch(f, s);
+                    exits.push_back({s, 1});
+                    f.outs = g.outs;
+                }
+                f.outs.insert(f.outs.end(), exits.begin(), exits.end());
+            }
+            return f;
+        }
+        }
+    }
+};
+
+// epsilon closure of `seed` (sorted, unique result).  BOL edges are followed only at the start of the line, EOL edges
+// only when `at_eol`.  *match = MATCH was reached.
+void closure(const Nfa &N, std::vector<int> seed, bool at_bol, bool at_eol, std::vector<int> *out, bool *match)
+{
+    std::vector<char> seen(N.st.size(), 0);
+    out->clear();
+    *match = false;
+    while (!seed.empty())
+    {
+        int s = seed.back();
+        seed.pop_back();
+        if (s < 0 || seen[s]) continue;
+        seen[s] = 1;
+        const NState &x = N.st[s];
+        switch (x.kind)
+        {
+        case NState::CHAR: out->push_back(s); break;
+        case NState::MATCH: *match = true; break;
+        case NState::SPLIT: seed.push_back(x.out); seed.push_back(x.out1); break;
+        case NState::BOL: if (at_bol) seed.push_back(x.out); break;
+        case NState::EOL:
+            if (at_eol) seed.push_back(x.out);
+            else out->push_back(s); // kept: the line may end right here
+            break;
+        }
+    }
+    std::sort(out->begin(), out->end());
+}
+
+} // namespace
+
+// The regular expression krep hands to regcomp (krep.c:2081-2145 and 2539-2600): patterns are read as C strings.
+bool regex_source(const search_params_t *P, std::string *out)
+{
+    if (!P || P->num_patterns == 0 || !P->patterns) return false;
+    std::string r;
+    if (P->num_patterns > 1)
+    {
+        for (size_t k = 0; k < P->num_patterns; k++)
+        {
+            const char *p = P->patterns[k] ? P->patterns[k] : "";
+            r += P->whole_word ? std::string("(\\b") + p + "\\b)" : std::string("(") + p + ")";
+            if (k + 1 < P->num_patterns) r += "|";
+        }
+    }
+    else
+    {
+        const char *p = P->patterns[0] ? P->patterns[0] : "";
+        r = P->whole_word ? std::string("\\b") + p + "\\b" : std::string(p);
+    }
+    *out = r;
+    return true;
+}
+
+int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why)
+{
+    if (MB_CUR_MAX != 1)
+    {
+        // krep never calls setlocale: its regexes are C-locale regexes.  A host running in a multibyte locale compiled
+        // a regex whose '.' and brackets match characters of several bytes, which a byte automaton does not model.
+        *why = "the process runs in a multibyte locale";
+        return -1;
+    }
+    Parser ps(re, icase);
+    int root = ps.parse_alt();
+    if (root >= 0 && ps.i != re.size()) root = ps.refuse("unmatched ')'");
+    if (root < 0)
+    {
+        *why = ps.why;
+        return -1;
+    }
+    Nfa N;
+    Nfa::Frag f = N.build(ps.nodes, root);
+    int m = N.add(NState::MATCH);
+    N.patch(f, m);
+    if (N.too_big)
+    {
+        *why = "the automaton is too large";
+        return -1;
+    }
+    const int start = f.in;
+
+    // byte classes: bytes that every character set of the pattern treats alike; '\n' is a class of its own
+    std::map<std::vector<bool>, int> sig_class;
+    uint8_t cls[256];
+    for (int b = 0; b < 256; b++)
+    {
+        std::vector<bool> sig(N.sets.size() + 1);
+        for (size_t k = 0; k < N.sets.size(); k++) sig[k] = N.sets[k][b];
+        sig[N.sets.size()] = b == '\n';
+        auto it = sig_class.find(sig);
+        if (it == sig_class.end()) it = sig_class.emplace(sig, (int)sig_class.size()).first;
+        cls[b] = (uint8_t)it->second;
+    }
+    const int nc = (int)sig_class.size();
+    if (nc > 255)
+    {
+        *why = "too many byte classes";
+        return -1;
+    }
+    std::vector<int> rep(nc, 0); // one byte of each class
+    for (int b = 255; b >= 0; b--) rep[cls[b]] = b;
+
+    // subset construction of the unanchored line automaton [^\n]*R.  DFA state 0 = MATCHED (the line is flagged), 1 =
+    // DEAD (no match can start or end anywhere in the rest of the line); the line-start state comes next.
+    struct DState
+    {
+        std::vector<int> set;
+        bool bol;
+    };
+    std::vector<DState> states(2);
+    std::map<std::pair<std::vector<int>, bool>, int> index;
+    std::vector<std::vector<int>> next; // next[s][c]
+    std::vector<char> eol_acc;          // accepts when the line ends here
+    std::vector<int> restart;
+    bool restart_match = false;
+    closure(N, {start}, false, false, &restart, &restart_match);
+
+    auto intern = [&](std::vector<int> set, bool bol, bool matched) -> int {
+        if (matched) return 0;
+        auto key = std::make_pair(set, bol);
+        auto it = index.find(key);
+        if (it != index.end()) return it->second;
+        states.push_back(DState{std::move(set), bol});
+        index.emplace(key, (int)states.size() - 1);
+        return (int)states.size() - 1;
+    };
+    std::vector<int> s0;
+    bool m0 = false;
+    closure(N, {start}, true, false, &s0, &m0);
+    const int start_state = intern(s0, true, m0);
+    const size_t budget_entries = REGEX_TABLE_BYTES / sizeof(uint16_t);
+    next.assign(2, std::vector<int>(nc, 0));
+    eol_acc.assign(2, 0);
+    eol_acc[0] = 1;
+    for (int c = 0; c < nc; c++) next[1][c] = 1;
+    for (size_t s = 2; s < states.size(); s++)
+    {
+        if (states.size() * (size_t)nc > budget_entries || states.size() > REGEX_MAX_STATES)
+        {
+            *why = "the automaton has too many states";
+            return -1;
+        }
+        const std::vector<int> set = states[s].set;
+        const bool bol = states[s].bol;
+        // end of line here?
+        {
+            std::vector<int> seed = set, tmp;
+            if (bol) seed.push_back(start);
+            bool acc = false;
+            closure(N, seed, bol, true, &tmp, &acc);
+            eol_acc.push_back(acc ? 1 : 0);
+        }
+        std::vector<int> row(nc, 1);
+        for (int c = 0; c < nc; c++)
+        {
+            if (c == cls['\n']) continue; // the kernel reads the '\n' column as "accepts at end of line"
+            const int b = rep[c];
+            std::vector<int> moved = restart;
+            for (int x : set)
+                if (N.st[x].kind == NState::CHAR && N.sets[N.st[x].set][b]) moved.push_back(N.st[x].out);
+            std::vector<int> cl;
+            bool mt = false;
+            closure(N, moved, false, false, &cl, &mt);
+            row[c] = intern(cl, false, mt);
+        }
+        next.push_back(row);
+    }
+    const int S = (int)states.size();
+    // states from which no match is reachable within the line behave like DEAD
+    std::vector<char> live(S, 0);
+    live[0] = 1;
+    for (bool changed = true; changed;)
+    {
+        changed = false;
+        for (int s = 2; s < S; s++)
+        {
+            if (live[s]) continue;
+            bool l = eol_acc[s];
+            for (int c = 0; c < nc && !l; c++) l = c != cls['\n'] && live[next[s][c]];
+            if (l) live[s] = 1, changed = true;
+        }
+    }
+    D->nclasses = (uint32_t)nc;
+    D->nl_class = cls['\n'];
+    memcpy(D->cls, cls, 256);
+    D->nstates = (uint32_t)S;
+    D->start = (uint32_t)((live[start_state] ? start_state : 1) * nc);
+    D->trans.assign((size_t)S * nc, 0);
+    for (int s = 0; s < S; s++)
+        for (int c = 0; c < nc; c++)
+        {
+            int t;
+            if (s == 0) t = 0;
+            else if (c == cls['\n']) t = eol_acc[s] ? 0 : 1;
+            else t = live[next[s][c]] ? next[s][c] : 1;
+            D->trans[(size_t)s * nc + c] = (uint16_t)(t * nc); // entries are row offsets: next = trans[row + class]
+        }
+    D->widened = ps.widened || N.widened;
+    return 0;
+}
+
+// The line filter run on the host — what k_regex_lines computes, without the kernel's long-line bound.
+void regex_lines_host(const RegexDfa &D, const char *t, size_t n, std::vector<uint64_t> *out)
+{
+    out->clear();
+    const uint32_t nc = D.nclasses, dead = nc;
+    size_t p = 0;
+    while (p < n)
+    {
+        uint32_t row = D.start;
+        size_t q = p;
+        for (; q < n && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
+        if (row > dead) row = D.trans[row + D.nl_class]; // end of line (or of the text)
+        if (row == 0) out->push_back(p);
+        const void *nl = q < n ? memchr(t + q, '\n', n - q) : nullptr;
+        if (!nl) break;
+        p = (size_t)((const char *)nl - t) + 1;
+    }
+}
+
+} // namespace kb

@@ -443,7 +443,7 @@ __global__ void __launch_bounds__(1024) k_count_finish(const LineRec *recs, uint
 // kernels' tail sub-search recounts a straddling line, tag-mode -w plans need the cursor walk, prefix plans are -o.)
 bool count_lines_eligible(const Plan *plan, const search_params_t *P, int algo)
 {
-    if (!P->count_lines_mode || plan->is_ac || plan->emit_len != plan->m || plan->whole_word == 2) return false;
+    if (!P->count_lines_mode || plan->is_ac || plan->is_regex || plan->emit_len != plan->m || plan->whole_word == 2) return false;
     if (plan->pattern.find('\n') != std::string::npos) return false;
     return algo == KREP_B200_ALGO_BMH || algo == KREP_B200_ALGO_KMP || algo == KREP_B200_ALGO_MEMCHR ||
            algo == KREP_B200_ALGO_MEMCHR_SHORT || algo == KREP_B200_ALGO_SSE42;

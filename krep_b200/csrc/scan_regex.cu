@@ -1,0 +1,170 @@
+// scan_regex.cu — the line filter of -E searches on sm_90a.
+//
+// One question per line: can the regex match somewhere in it?  The line automaton (regex_dfa.cpp) answers it; the
+// flagged lines go back as keys (global line start << LIT_TAG_BITS) through the engine's occurrence list, and glibc's
+// regexec confirms them on the host (replay_regex, semantics.cpp).  Nothing here computes a match offset.
+//
+//   * the transition table (row-offset entries, <= 32 KiB) and the 256-byte class map live in shared memory;
+//   * a thread owns a segment of RX_SEG bytes of the shard's owned range, and in it every line whose first byte lies
+//     in the segment (a segment starts a line only when the byte before it is '\n' — at a shard edge that byte is the
+//     shard's prev_byte, and there is none at the start of the text);
+//   * the owner runs the automaton from the line's first byte, across its segment's end if needed, up to the line's
+//     newline.  Once the line is MATCHED (flagged) or DEAD (cannot match any more) it skips to the newline 16 bytes
+//     at a time;
+//   * a line that runs more than REGEX_HALO bytes past its segment, or past the shard's readable bytes, is flagged
+//     unverified: always safe, glibc then looks at it on the host;
+//   * the text is read as aligned 16-byte vectors held in registers (one LDG.128 per 16 bytes of a thread's walk).
+//
+// Work per byte: one class lookup and one transition lookup in shared memory.
+#include <cooperative_groups.h>
+#include "common.h"
+#include "engine.h"
+
+namespace cg = cooperative_groups;
+
+namespace kb {
+
+namespace {
+
+constexpr int RX_THREADS = 256;
+constexpr uint32_t RX_SEG = 256; // bytes of owned range per thread
+
+// The aligned 16 bytes around the last position read, in registers.
+struct Window
+{
+    const uint8_t *text;
+    uint64_t avail;
+    uint64_t base;
+    uint4 v;
+
+    __device__ __forceinline__ void load(uint64_t b)
+    {
+        base = b;
+        if (b + 16 <= avail)
+        {
+            v = __ldg(reinterpret_cast<const uint4 *>(text + b));
+            return;
+        }
+        uint32_t w[4] = {0, 0, 0, 0};
+#pragma unroll
+        for (int k = 0; k < 16; k++)
+            if (b + k < avail) w[k >> 2] |= (uint32_t)text[b + k] << ((k & 3) * 8);
+        v = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    __device__ __forceinline__ uint32_t at(uint64_t q)
+    {
+        const uint64_t b = q & ~15ull;
+        if (b != base) load(b);
+        const uint32_t i = (uint32_t)q & 15u;
+        const uint32_t w = (i & 8) ? ((i & 4) ? v.w : v.z) : ((i & 4) ? v.y : v.x);
+        return (w >> ((i & 3) * 8)) & 0xFFu;
+    }
+};
+
+__device__ __forceinline__ bool has_newline(uint4 v)
+{
+    auto z = [](uint32_t x) {
+        x ^= 0x0A0A0A0Au;
+        return (x - 0x01010101u) & ~x & 0x80808080u;
+    };
+    return (z(v.x) | z(v.y) | z(v.z) | z(v.w)) != 0;
+}
+
+// Position of the first '\n' in [q, end), or end.
+__device__ __forceinline__ uint64_t next_newline(Window &W, uint64_t q, uint64_t end)
+{
+    while (q < end)
+    {
+        if ((q & 15) == 0 && q + 16 <= end)
+        {
+            if (W.base != q) W.load(q);
+            if (!has_newline(W.v))
+            {
+                q += 16;
+                continue;
+            }
+        }
+        if (W.at(q) == '\n') return q;
+        q++;
+    }
+    return end;
+}
+
+__global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constant__ RegexLaunch a)
+{
+    extern __shared__ uint4 s_raw[];
+    uint16_t *s_tab = reinterpret_cast<uint16_t *>(s_raw);
+    const uint32_t tab_words = (a.ntrans + 7) & ~7u; // the class map follows the table, 16-byte aligned
+    const uint32_t nvec = (tab_words * 2 + 256) / 16;
+    const uint4 *src = reinterpret_cast<const uint4 *>(a.trans);
+    for (uint32_t i = threadIdx.x; i < nvec; i += blockDim.x) s_raw[i] = src[i];
+    __syncthreads();
+    const uint8_t *s_cls = reinterpret_cast<const uint8_t *>(s_tab + tab_words);
+    const uint32_t dead = a.nclasses, nl = a.nl_class;
+
+    const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
+    const uint64_t nseg = (own + RX_SEG - 1) / RX_SEG;
+    Window W{a.text, a.avail_len, ~0ull, make_uint4(0, 0, 0, 0)};
+    for (uint64_t sg = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; sg < nseg; sg += (uint64_t)gridDim.x * blockDim.x)
+    {
+        const uint64_t sb = a.own_begin + sg * RX_SEG;
+        const uint64_t se = sb + RX_SEG < a.own_end ? sb + RX_SEG : a.own_end;
+        const uint64_t limit = se + REGEX_HALO < a.avail_len ? se + REGEX_HALO : a.avail_len;
+        uint64_t p = sb;
+        const int before = sb == 0 ? a.prev_byte : (int)W.at(sb - 1);
+        if (before >= 0 && before != '\n')
+        {
+            p = next_newline(W, sb, se) + 1; // the line in progress belongs to an earlier segment
+            if (p > se) continue;
+        }
+        while (p < se)
+        {
+            uint32_t row = a.start;
+            uint64_t q = p;
+            while (row > dead && q < limit)
+            {
+                const uint32_t b = W.at(q);
+                if (b == '\n') break;
+                row = s_tab[row + s_cls[b]];
+                q++;
+            }
+            bool flag;
+            if (row <= dead) flag = row == 0;                                           // MATCHED / DEAD
+            else if (q < limit || (q == a.avail_len && a.next_byte < 0)) flag = s_tab[row + nl] == 0; // end of the line
+            else flag = true;                                                        // line not seen to its end: unverified
+            if (flag)
+            {
+                cg::coalesced_group g = cg::coalesced_threads();
+                unsigned long long base = 0;
+                if (g.thread_rank() == 0) base = atomicAdd(a.counter, (unsigned long long)g.size());
+                base = g.shfl(base, 0) + g.thread_rank();
+                if (base < a.cap) a.out[base] = (a.global_offset + p) << LIT_TAG_BITS;
+            }
+            if (row <= dead) q = next_newline(W, q, limit);
+            if (q >= limit) break; // the next line starts beyond this thread's reach, hence beyond its segment
+            p = q + 1;
+        }
+    }
+}
+
+} // namespace
+
+void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
+{
+    const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
+    {
+        cudaGetLastError();
+        per_sm = 1;
+    }
+    const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
+    const uint64_t blocks_needed = (own + (uint64_t)RX_SEG * RX_THREADS - 1) / ((uint64_t)RX_SEG * RX_THREADS);
+    const uint64_t resident = (uint64_t)sm_count * per_sm;
+    const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
+    trace("regex: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", grid, RX_THREADS, per_sm, smem);
+    k_regex_lines<<<grid, RX_THREADS, smem, s>>>(a);
+    count_launch();
+}
+
+} // namespace kb

@@ -9,7 +9,9 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <cstdio>
 #include <omp.h>
+#include <regex.h>
 #include <vector>
 #include "common.h"
 
@@ -561,6 +563,129 @@ uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *re
         }
     }
     return found;
+}
+
+// ---- regex_search (krep.c:1389-1579) over the lines the device flagged ----------------------------------------------
+// Under REG_NEWLINE no match contains a '\n' (regex_dfa.cpp refuses character sets that hold one), so the reference loop
+// is unchanged if (1) the cursor skips every line the filter did not flag — glibc finds no match starting there, from
+// the line start or from any position inside it — and (2) each regexec call is clipped to the run of consecutive
+// flagged lines the cursor is in: [cur, E) with E the byte after the run's last newline, and REG_NOTEOL when E is not
+// the end of the text, so that '$' cannot match at a false end of string.  Every match, and every -w / -c / -m
+// decision, is glibc's own on the caller's regex_t.  r.keys are the flagged line starts (ascending, global offsets).
+uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res)
+{
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0;
+    if (!P->compiled_regex) return 0;
+    const regex_t *regex = (const regex_t *)P->compiled_regex;
+    const char *t = r.text;
+    const size_t n = r.text_len;
+    if (n == 0)
+    {
+        regmatch_t m;
+        if (regexec(regex, "", 1, &m, 0) == 0)
+        {
+            if (P->count_lines_mode) return 1;
+            if (P->track_positions && res) result_push(res, 0, 0);
+            return 1;
+        }
+        return 0;
+    }
+    // krep.c:1422 passes compilation flags as execution flags: REG_NEWLINE has the value of REG_STARTEND and REG_ICASE
+    // the value of REG_NOTEOL.  Passed on exactly as the reference does.
+    const int base_eflags = REG_STARTEND | REG_NEWLINE | (P->case_sensitive ? 0 : REG_ICASE);
+    const size_t max_count = P->max_count;
+    const size_t RUN_MAX = (size_t)1 << 30; // regoff_t is an int: a run is cut (at a line start) before it gets near 2^31
+    auto key_pos = [&](size_t j) { return (size_t)((r.keys[j] >> LIT_TAG_BITS) - r.base); };
+    auto after_line = [&](size_t s) {
+        const size_t e = line_end(t, n, s);
+        return e < n ? e + 1 : n;
+    };
+    size_t ki = 0, run_end = 0, cur = 0, last_line = SIZE_MAX;
+    uint64_t count = 0;
+    while (cur < n)
+    {
+        if (cur >= run_end)
+        {
+            // the next run: the first flagged line that ends after the cursor, and the flagged lines right behind it
+            size_t s = 0, e = 0;
+            bool found = false;
+            while (ki < r.n && !found)
+            {
+                s = key_pos(ki++);
+                if (s >= n) break;
+                e = after_line(s);
+                found = e > cur;
+            }
+            if (!found)
+            {
+                // no flagged line left.  A text that ends with '\n' still has an empty string after it, where the
+                // reference's search from the cursor can end with an empty match (^ or $ at the end of the text)
+                if (t[n - 1] != '\n') break;
+                s = e = n;
+            }
+            const size_t run_start = s;
+            while (ki < r.n && e < n && key_pos(ki) == e && e - run_start < RUN_MAX) e = after_line(key_pos(ki++));
+            run_end = e;
+            if (cur < run_start) cur = run_start;
+        }
+        regmatch_t pmatch[1];
+        pmatch[0].rm_so = 0;
+        pmatch[0].rm_eo = (regoff_t)(run_end - cur);
+        const bool at_line_start = cur == 0 || t[cur - 1] == '\n';
+        const int eflags = base_eflags | (at_line_start ? 0 : REG_NOTBOL) | (run_end < n ? REG_NOTEOL : 0);
+        const int rc = regexec(regex, t + cur, 1, pmatch, eflags);
+        if (rc != 0)
+        {
+            if (rc == REG_NOMATCH)
+            {
+                cur = run_end; // nothing more in this run: on to the next one
+                continue;
+            }
+            char ebuf[256];
+            regerror(rc, regex, ebuf, sizeof(ebuf));
+            fprintf(stderr, "krep: Regex execution error: %s\n", ebuf);
+            return count;
+        }
+        if (pmatch[0].rm_so == -1 || pmatch[0].rm_eo == -1)
+        {
+            fprintf(stderr, "krep: Warning: regexec returned success but invalid offsets.\n");
+            break;
+        }
+        const size_t so = (size_t)pmatch[0].rm_so, eo = (size_t)pmatch[0].rm_eo;
+        if (eo < so)
+        {
+            fprintf(stderr, "krep: Warning: regexec returned eo < so.\n");
+            cur = std::min(cur + so + 1, n);
+            continue;
+        }
+        const size_t start = cur + so, end = cur + eo;
+        if (P->whole_word && ((start > 0 && is_word_c((unsigned char)t[start - 1])) || (end < n && is_word_c((unsigned char)t[end]))))
+        {
+            cur = std::min(cur + so + 1, n); // krep.c:1487-1501
+            continue;
+        }
+        if (P->count_lines_mode)
+        {
+            const size_t ls = line_start(t, n, start);
+            if (ls != last_line)
+            {
+                count++;
+                last_line = ls;
+                if (count >= max_count) break;
+                cur = after_line(ls); // krep.c:1515-1519: on to the next line
+                continue;
+            }
+        }
+        else
+        {
+            count++;
+            if (P->track_positions && res) result_push(res, start, end);
+        }
+        if (count >= max_count) break;
+        const size_t next = cur + (so == eo ? so + 1 : eo);
+        cur = next > n ? n : next;
+    }
+    return count;
 }
 
 } // namespace kb

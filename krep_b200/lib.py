@@ -22,6 +22,7 @@ SEARCH_ENTRIES = {
     "avx512": "krep_b200_simd_avx512_search",
     "aho_corasick": "krep_b200_aho_corasick_search",
     "neon": "krep_b200_neon_search",
+    "regex": "krep_b200_regex_search",
 }
 
 _lib = None
@@ -99,6 +100,9 @@ def load():
     L.krep_b200_search_shards.restype = C.c_uint64
     L.krep_b200_export_keys.argtypes = [C.POINTER(DeviceResult), C.c_void_p, C.c_uint64, C.c_void_p]
     L.krep_b200_export_keys.restype = C.c_int
+    L.krep_b200_regex_filter_host.argtypes = [C.POINTER(SearchParams), C.c_void_p, C.c_size_t, C.POINTER(C.c_uint64), C.c_uint64,
+                                              C.POINTER(C.c_int)]
+    L.krep_b200_regex_filter_host.restype = C.c_int64
     L.krep_b200_last_kernel_ms.restype = C.c_float
     L.krep_b200_launch_count.restype = C.c_uint64
     for n in ("krep_b200_ac_key_end", "krep_b200_ac_key_start"):

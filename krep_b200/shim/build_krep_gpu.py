@@ -13,8 +13,11 @@ binaries built from the reference sources).
      --algo globals into the library and returns the krep_b200_* function;
   3. search_file hands the whole file to ONE search call (krep.c:2765: the single-chunk branch) — the GPU
      does its own tiling, and the result is the reference's -t 1 result rather than its multi-thread
-     chunk-edge artefacts (SURVEY §8 a12);
-  4. main calls krep_b200_warmup() right before it starts searching (krep.c:3818), and the file is mapped
+     chunk-edge artefacts (SURVEY §8 a12).  -E searches too, when the library takes the pattern (krep's
+     regex chunks do not overlap, so a match across a chunk edge would be lost); a refused pattern keeps
+     krep's own threading;
+  4. main calls krep_b200_warmup() right before it starts searching (krep.c:3818; for -E only when the library
+     takes the pattern), and the file is mapped
      without MAP_POPULATE for literal searches (krep.c:2679): CUDA start-up overlaps the file handling.
 
 The output binary is oracle/_ref/krep_gpu: same CLI, same output code, GPU scan.
@@ -45,12 +48,14 @@ def patched_source():
                         "static search_func_t select_search_algorithm_cpu(const search_params_t *params)\n{",
                         "select_search_algorithm")
     src = _replace_once(src, "    run_single_thread_inline = (actual_thread_count == 1);",
-                        "    if (!current_params.use_regex)\n        actual_thread_count = 1; /* krep_b200: one call per file */\n"
+                        "    if (!current_params.use_regex || krep_b200_select_search_algorithm(&current_params))\n"
+                        "        actual_thread_count = 1; /* krep_b200: one call per file */\n"
                         "    run_single_thread_inline = (actual_thread_count == 1);", "the chunk count")
     # 4. start-up: the GPU context comes up on a background thread while search_file opens and maps the file, and the
     #    mapping is not pre-populated by one kernel thread (the library's staging threads fault it in, in parallel)
     src = _replace_once(src, "    // --- Execute Search ---\n    int exit_code = 1;",
-                        "    if (!params.use_regex)\n        krep_b200_warmup(); /* krep_b200: context creation overlaps the file handling */\n"
+                        "    if (!params.use_regex || krep_b200_select_search_algorithm(&params))\n"
+                        "        krep_b200_warmup(); /* krep_b200: context creation overlaps the file handling */\n"
                         "    // --- Execute Search ---\n    int exit_code = 1;", "the warm-up call")
     src = _replace_once(src, "int mmap_flags_populate = mmap_base_flags | MAP_POPULATE;",
                         "int mmap_flags_populate = mmap_base_flags | ((current_params.use_regex || getenv(\"KREP_B200_MAP_POPULATE\")) ? MAP_POPULATE : 0); /* krep_b200 */",
