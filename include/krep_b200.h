@@ -144,6 +144,11 @@ uint64_t krep_b200_neon_search(const search_params_t *, const char *, size_t, ma
  * Accepted: literals and escaped punctuation, '.', bracket expressions with ranges, negation and the classes alpha,
  * digit, alnum, upper, lower, blank, punct, print, graph, xdigit; ^ $ ( ) | * + ? {m} {m,} {m,n} {,n} (counts <= 255);
  * \w; \b \B \< \> (the filter treats them as empty: a wider answer, never a narrower one).
+ * -c without -w (count_lines_mode) on a pattern whose line automaton is exact (no word assertion, no -i bracket that
+ * case folding widens, no anchor inside a repeated group) is counted on the GPU: lines the automaton decides there are
+ * counted in the scan, and regexec sees only the lines it cannot decide (a line longer than the scan's reach, and the
+ * text's last line).  The count is the same; KREP_B200_NO_FUSED_COUNT=1 turns this off
+ * (krep_b200_regex_count_mode tells which path a call takes).
  * Refused (the pattern stays with the host's regex_search): back-references, \` \', \s \S \W, [[:space:]],
  * [[:cntrl:]], collating elements, any character set that holds '\n' or a newline in the pattern, non-ASCII pattern
  * bytes, unknown escapes, a process running in a multibyte locale (krep itself never calls setlocale), and automata
@@ -354,6 +359,15 @@ uint64_t krep_b200_replay(int algo, const search_params_t *params, bool only_mat
  * automaton accepts more than the regex.  No search entry point calls it. */
 int64_t krep_b200_regex_filter_host(const search_params_t *params, const char *text, size_t n, uint64_t *line_starts,
                                     uint64_t cap, int *widened);
+
+/* Test hook: which path a -E call with params takes — 1 when it is a -c call counted on the device (see
+ * krep_b200_regex_search), 0 when its lines go through regexec, -1 when the pattern is refused. */
+int krep_b200_regex_count_mode(const search_params_t *params);
+/* Test hook, host only: the fused -E -c on the CPU — the line automaton decides every line it can within `reach` bytes
+ * of the line's start (UINT64_MAX: no bound), and the lines it leaves uncertain (out of reach, or holding the text's
+ * last byte) go to regexec as in krep_b200_regex_search.  Returns the count, or -1 when the pattern is refused or a
+ * -c call with params would not be counted on the device whatever KREP_B200_NO_FUSED_COUNT says. */
+int64_t krep_b200_regex_count_host(const search_params_t *params, const char *text, size_t n, uint64_t reach);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

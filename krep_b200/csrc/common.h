@@ -73,10 +73,14 @@ struct RegexDfa
     uint8_t cls[256];
     std::vector<uint16_t> trans;
     bool widened = false; // the automaton accepts more than the regex (word assertions, -i brackets)
+    bool count_exact = false; // its per-line answer is glibc's: -c may be counted on the device (DESIGN §12.1)
 };
 bool regex_source(const search_params_t *P, std::string *out); // the string krep compiles (krep.c:2081-2145)
 int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why); // 0, or -1 = refused (*why)
 void regex_lines_host(const RegexDfa &D, const char *text, size_t n, std::vector<uint64_t> *line_starts);
+// The count mode of k_regex_lines on the host, every line walked at most `reach` bytes: returns the lines decided
+// MATCHED and stores the uncertain line starts (live at the bound, or holding the text's last byte) in *uncertain.
+uint64_t regex_count_lines_host(const RegexDfa &D, const char *text, size_t n, uint64_t reach, std::vector<uint64_t> *uncertain);
 
 struct RegexLaunch
 {
@@ -88,6 +92,7 @@ struct RegexLaunch
     uint64_t *out;
     uint64_t cap;
     unsigned long long *counter;
+    unsigned long long *line_count; // count mode (-c): lines decided MATCHED on the device; nullptr = filter mode
 };
 
 struct AcDevTables;  // scan_multi.cu: one device's copy of a pattern set's tables
@@ -158,7 +163,9 @@ static constexpr uint64_t LB_SAME_AS_NEXT = ~0ull - 1; // no newline between thi
 static constexpr uint64_t LB_OUTSIDE_SHARD = ~0ull - 2; // the line continues into a neighbouring shard
 
 // Launch one shard scan on `stream` of the device context; appends to that device's key list (no counter reset).
-int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0);
+// regex_lines (regex plans only): run k_regex_lines in count mode, adding the lines it decides MATCHED there.
+int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0,
+                unsigned long long *regex_lines = nullptr);
 // literal kernels (scan_literal.cu)
 void launch_literal(const Plan *plan, const LitDevParams &p, int sm_count, cudaStream_t s);
 // multi kernels (scan_multi.cu)

@@ -578,7 +578,8 @@ Plan *plan_build(const search_params_t *P, int algo, bool only_matching)
 // ---------------------------------------------------------------------------------------------
 // shard scan
 // ---------------------------------------------------------------------------------------------
-int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot)
+int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot,
+                unsigned long long *regex_lines)
 {
     if (((uintptr_t)sh->d_text & 15) != 0)
     {
@@ -606,6 +607,7 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.out = E.d_list[slot];
         a.cap = want_positions ? E.key_cap : 0;
         a.counter = slot_counter(E, slot);
+        a.line_count = regex_lines;
         launch_regex(a, E.sm_count, stream);
         return 0;
     }

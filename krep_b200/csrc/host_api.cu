@@ -308,6 +308,8 @@ struct RangeJob
     bool pinned = false;
     bool count_lines = false; // fused -c: every chunk leaves one line record instead of occurrence keys
     std::vector<uint64_t> line_recs; // (lines, flags) per chunk, text order
+    bool regex_count = false; // fused -E -c: every chunk adds its device-decided matching lines and leaves its uncertain keys
+    uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
     // results
     int rc = 0;
     ScanOut so;
@@ -333,12 +335,15 @@ static int stream_range(RangeJob &J)
     if (!J.pinned && ensure_stage(E, std::min(chunk, span) + halo + 64, nslots) != 0) return -2;
     if (J.want_positions && ensure_keys(E, 1) != 0) return -2;
     if (J.count_lines && ensure_line_out(E, nchunks) != 0) return -2;
+    if (J.regex_count && ensure_line_out(E, 1) != 0) return -2; // the range's line counter: d_line_out[0]
+    unsigned long long *d_regex_lines = J.regex_count ? (unsigned long long *)E.d_line_out : nullptr;
     reset_kernel_ms();
     const int slot = 0;
     for (int attempt = 0; attempt < 3; attempt++)
     {
         CKH(cudaStreamWaitEvent(E.scan_stream, E.ev_done[slot], 0));
         if (reset_counter(E, slot, E.scan_stream) != 0) return -2;
+        if (d_regex_lines) CKH(cudaMemsetAsync(d_regex_lines, 0, sizeof(unsigned long long), E.scan_stream)); // also on a re-stage
         for (size_t c = 0; c < nchunks; c++)
         {
             const size_t off = J.begin + c * chunk, len = std::min(chunk, J.end - off);
@@ -370,13 +375,14 @@ static int stream_range(RangeJob &J)
             cudaEvent_t a = pool_event(E, 2 * c), b = pool_event(E, 2 * c + 1);
             CKH(cudaEventRecord(a, E.scan_stream));
             int rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
-                                   : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot);
+                                   : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
             CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
         }
         CKH(cudaGetLastError());
         if (!J.count_lines && finish_scan(E, slot, J.want_positions, E.scan_stream) != 0) return -2;
+        if (d_regex_lines) CKH(cudaMemcpyAsync(E.h_line_out, d_regex_lines, sizeof(uint64_t), cudaMemcpyDeviceToHost, E.scan_stream));
         CKH(cudaStreamSynchronize(E.scan_stream));
         if (!J.count_lines) CKH(cudaEventSynchronize(E.ev_done[slot])); // k_finish runs on the finish stream
         for (auto &s : E.stage) s.in_flight = false;
@@ -392,6 +398,7 @@ static int stream_range(RangeJob &J)
             J.so = ScanOut();
             return 0;
         }
+        if (J.regex_count) J.regex_lines = E.h_line_out[0];
         const uint64_t cnt = E.h_pack[slot][0];
         J.so = ScanOut();
         J.so.count = cnt;
@@ -455,8 +462,11 @@ struct HostScan
     const uint64_t *keys = nullptr;
     uint64_t nkeys = 0;
     std::vector<uint64_t> merged; // backing store when several devices contributed
+    uint64_t regex_lines = 0;     // fused -E -c: lines decided MATCHED on the devices (the keys are the uncertain lines)
 };
 
+// count_lines: the fused -c of the plan — a line record per chunk for literals; for regex plans a device line count per
+// range next to the keys of the uncertain lines (want_positions must then be set).
 static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want_positions, HostScan *hs, bool count_lines = false)
 {
     const bool pinned = is_pinned(text);
@@ -488,7 +498,8 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.end = std::min((i + 1) * per * chunk, n);
         J.want_positions = want_positions;
         J.pinned = pinned;
-        J.count_lines = count_lines;
+        J.count_lines = count_lines && !plan->is_regex;
+        J.regex_count = count_lines && plan->is_regex;
     }
     trace("search: %zu bytes (%s host memory), %zu device(s), %zu range(s), chunk %zu MiB", n, pinned ? "pinned" : "pageable", D, R,
           chunk >> 20);
@@ -553,7 +564,8 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
     hs->count = 0;
     hs->keys = nullptr;
     hs->nkeys = 0;
-    if (count_lines)
+    hs->regex_lines = 0;
+    if (count_lines && !plan->is_regex)
     {
         // chunk records of all ranges, in text order -> matching lines (a line cut by a chunk / range / device edge is
         // counted on both sides and subtracted once)
@@ -562,7 +574,11 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         hs->count = combine_line_records(all.data(), all.size() / 2);
         return 0;
     }
-    for (auto &J : jobs) hs->count += J.so.count;
+    for (auto &J : jobs)
+    {
+        hs->count += J.so.count;
+        hs->regex_lines += J.regex_lines; // every line is decided by one range: the counts add up
+    }
     if (!want_positions) return 0;
     for (auto &J : jobs)
     {
@@ -576,7 +592,7 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         hs->nkeys = jobs[0].so.stored;
         return 0;
     }
-    // ranges are in text order: literal keys concatenate in order, pattern-set keys (ordered by end, owned by start) need
+    // ranges are in text order: literal and regex keys concatenate in order, pattern-set keys (ordered by end, owned by start) need
     // the merge around each cut
     std::vector<const uint64_t *> lists;
     std::vector<uint64_t> counts;
@@ -752,9 +768,38 @@ static uint64_t run_search(int entry_algo, const search_params_t *P, const char 
     return ret;
 }
 
+// Can a -E call with these params count its lines on the device?  -c without -w (count_lines_mode, not -co) on a plan
+// whose per-line answer is glibc's.  KREP_B200_NO_FUSED_COUNT is not looked at here.
+static bool regex_count_exact(const search_params_t *P, const Plan *plan)
+{
+    return P->count_lines_mode && !P->whole_word && plan->rx->count_exact;
+}
+
+static bool regex_count_fused(const search_params_t *P, const Plan *plan)
+{
+    return regex_count_exact(P, plan) && !getenv("KREP_B200_NO_FUSED_COUNT");
+}
+
+// Fused -E -c: the answer is  min(lines the device decided MATCHED + replay_regex over the uncertain lines, max_count).
+// Why this is the reference's count: without -w and -o the loop of krep.c:1389-1579 calls regexec only at line starts
+// (after a counted line the cursor jumps to the next line start; with no match left the loop ends) and never with
+// REG_NOTBOL, and under REG_NEWLINE no match contains a '\n'.  So a line is counted exactly when glibc finds a match in
+// it from its start, each line independently of the others — which the automaton of a count_exact plan decides — and
+// the -m limit only caps the total.  Two answers depend on the end of the text rather than on one line: '$' cannot
+// match at the end of the text under -i (REG_ICASE passed as an execution flag is REG_NOTEOL), and a text that ends in
+// '\n' holds an empty string at n that is counted when the last line was not and the regex matches there.  The line
+// holding the text's last byte is always among the uncertain keys, so both are decided inside glibc's last run, as in
+// the reference; skipping the lines counted on the device changes nothing for the runs in between, since each run starts
+// at a line start.
+static uint64_t regex_count_total(const search_params_t *P, uint64_t device_lines, const Replay &uncertain)
+{
+    return std::min<uint64_t>(device_lines + replay_regex(P, uncertain, nullptr), P->max_count);
+}
+
 // -E (regex_search, krep.c:1389): the device flags the lines the regex can match in (k_regex_lines), glibc's regexec
-// on the caller's regex_t confirms them and computes every offset (replay_regex).  The empty text is answered on the
-// host, as the reference does, without a launch.
+// on the caller's regex_t confirms them and computes every offset (replay_regex).  A -c call on a count_exact plan
+// counts the lines the device can decide there and leaves glibc only the uncertain ones (regex_count_total).  The empty
+// text is answered on the host, as the reference does, without a launch.
 static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, match_result_t *res)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
@@ -779,10 +824,18 @@ static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, 
         set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
         return 0;
     }
+    const bool fused = regex_count_fused(P, plan);
     HostScan hs;
-    if (stage_and_scan(plan, text, n, 1, &hs) != 0) return 0;
+    if (stage_and_scan(plan, text, n, 1, &hs, fused) != 0) return 0;
     r.keys = hs.keys;
     r.n = (size_t)hs.nkeys;
+    if (fused)
+    {
+        const uint64_t ret = regex_count_total(P, hs.regex_lines, r);
+        trace("search: regex -c fused: %llu lines counted on the device, %llu uncertain lines to regexec (%llu)",
+              (unsigned long long)hs.regex_lines, (unsigned long long)hs.nkeys, (unsigned long long)ret);
+        return ret;
+    }
     const uint64_t ret = replay_regex(P, r, res);
     trace("search: regex confirmed on %llu flagged lines (%llu)", (unsigned long long)hs.nkeys, (unsigned long long)ret);
     return ret;
@@ -1430,6 +1483,31 @@ int64_t krep_b200_regex_filter_host(const search_params_t *P, const char *text, 
     for (size_t i = 0; i < v.size() && i < cap; i++) line_starts[i] = v[i];
     if (widened) *widened = pl->rx->widened ? 1 : 0;
     return (int64_t)v.size();
+}
+
+// ---- test hooks: the fused -E -c, decided and run on the host ----
+int krep_b200_regex_count_mode(const search_params_t *P)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl) return -1;
+    return regex_count_fused(P, pl) ? 1 : 0;
+}
+
+int64_t krep_b200_regex_count_host(const search_params_t *P, const char *text, size_t n, uint64_t reach)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl || !regex_count_exact(P, pl)) return -1;
+    if (P->max_count == 0 || !P->compiled_regex) return 0; // run_regex's early returns
+    if (n == 0) return (int64_t)replay_regex(P, Replay{nullptr, 0, text, 0, 0}, nullptr);
+    if (!text) return 0;
+    std::vector<uint64_t> keys;
+    const uint64_t device_lines = regex_count_lines_host(*pl->rx, text, n, reach, &keys);
+    for (uint64_t &k : keys) k <<= LIT_TAG_BITS;
+    return (int64_t)regex_count_total(P, device_lines, Replay{keys.data(), keys.size(), text, n, 0});
 }
 
 } // extern "C"

@@ -618,6 +618,7 @@ int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *w
             D->trans[(size_t)s * nc + c] = (uint16_t)(t * nc); // entries are row offsets: next = trans[row + class]
         }
     D->widened = ps.widened || N.widened;
+    D->count_exact = !D->widened;
     return 0;
 }
 
@@ -638,6 +639,33 @@ void regex_lines_host(const RegexDfa &D, const char *t, size_t n, std::vector<ui
         if (!nl) break;
         p = (size_t)((const char *)nl - t) + 1;
     }
+}
+
+// The count mode of k_regex_lines (scan_regex.cu), one line at a time.  The kernel's walk ends REGEX_HALO bytes past its
+// thread's segment; here every line may be read `reach` bytes from its start (UINT64_MAX: to the end of the text), so a
+// small reach drives the uncertain-line path without a GPU.
+uint64_t regex_count_lines_host(const RegexDfa &D, const char *t, size_t n, uint64_t reach, std::vector<uint64_t> *uncertain)
+{
+    uncertain->clear();
+    const uint32_t dead = D.nclasses;
+    uint64_t counted = 0;
+    size_t p = 0;
+    while (p < n)
+    {
+        const size_t limit = reach < n - p ? p + (size_t)reach : n;
+        uint32_t row = D.start;
+        size_t q = p;
+        for (; q < limit && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
+        if (row > dead && q < limit) row = D.trans[row + D.nl_class]; // the walk stopped at the line's '\n'
+        if (row <= dead)
+            while (q < limit && t[q] != '\n') q++;
+        if (q >= limit || q + 1 == n) uncertain->push_back(p); // '\n' out of reach, or the text's last byte
+        else if (row == 0) counted++;
+        const void *nl = q < n ? memchr(t + q, '\n', n - q) : nullptr;
+        if (!nl) break;
+        p = (size_t)((const char *)nl - t) + 1;
+    }
+    return counted;
 }
 
 } // namespace kb

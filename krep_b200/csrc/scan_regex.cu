@@ -13,7 +13,9 @@
 //     at a time;
 //   * a line that runs more than REGEX_HALO bytes past its segment, or past the shard's readable bytes, is flagged
 //     unverified: always safe, glibc then looks at it on the host;
-//   * the text is read as aligned 16-byte vectors held in registers (one LDG.128 per 16 bytes of a thread's walk).
+//   * the text is read as aligned 16-byte vectors held in registers (one LDG.128 per 16 bytes of a thread's walk);
+//   * in count mode (fused -E -c) the same walk counts the lines it decides MATCHED (one atomic per warp) and emits
+//     keys for the uncertain lines only.
 //
 // Work per byte: one class lookup and one transition lookup in shared memory.
 #include <cooperative_groups.h>
@@ -90,6 +92,12 @@ __device__ __forceinline__ uint64_t next_newline(Window &W, uint64_t q, uint64_t
     return end;
 }
 
+// COUNT = false: the filter (one key per flagged line).  COUNT = true: the fused -c of plans whose per-line answer is
+// exact (RegexDfa::count_exact).  A line the walk decides (MATCHED or DEAD, or its '\n' read through the '\n' column)
+// is settled on the device, and a MATCHED one is counted; only the uncertain lines leave as keys: a line whose '\n' lies
+// beyond the walk's limit, and the line that holds the text's last byte (decided or not, so that both end-of-text
+// quirks of the reference stay with glibc: DESIGN §12.1).
+template <bool COUNT>
 __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constant__ RegexLaunch a)
 {
     extern __shared__ uint4 s_raw[];
@@ -105,6 +113,7 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
     const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
     const uint64_t nseg = (own + RX_SEG - 1) / RX_SEG;
     Window W{a.text, a.avail_len, ~0ull, make_uint4(0, 0, 0, 0)};
+    uint32_t counted = 0; // COUNT: lines of this thread decided MATCHED
     for (uint64_t sg = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; sg < nseg; sg += (uint64_t)gridDim.x * blockDim.x)
     {
         const uint64_t sb = a.own_begin + sg * RX_SEG;
@@ -129,9 +138,19 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
                 q++;
             }
             bool flag;
-            if (row <= dead) flag = row == 0;                                           // MATCHED / DEAD
-            else if (q < limit || (q == a.avail_len && a.next_byte < 0)) flag = s_tab[row + nl] == 0; // end of the line
-            else flag = true;                                                        // line not seen to its end: unverified
+            if constexpr (COUNT)
+            {
+                if (row > dead && q < limit) row = s_tab[row + nl]; // the walk stopped at the line's '\n'
+                if (row <= dead) q = next_newline(W, q, limit);
+                flag = q >= limit || (q + 1 == a.avail_len && a.next_byte < 0); // '\n' out of reach, or the text's last byte
+                counted += (!flag && row == 0) ? 1u : 0u;
+            }
+            else
+            {
+                if (row <= dead) flag = row == 0;                                           // MATCHED / DEAD
+                else if (q < limit || (q == a.avail_len && a.next_byte < 0)) flag = s_tab[row + nl] == 0; // end of the line
+                else flag = true;                                                        // line not seen to its end: unverified
+            }
             if (flag)
             {
                 cg::coalesced_group g = cg::coalesced_threads();
@@ -140,20 +159,28 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
                 base = g.shfl(base, 0) + g.thread_rank();
                 if (base < a.cap) a.out[base] = (a.global_offset + p) << LIT_TAG_BITS;
             }
-            if (row <= dead) q = next_newline(W, q, limit);
+            if constexpr (!COUNT)
+                if (row <= dead) q = next_newline(W, q, limit);
             if (q >= limit) break; // the next line starts beyond this thread's reach, hence beyond its segment
             p = q + 1;
         }
+    }
+    if constexpr (COUNT)
+    {
+        // every thread of the block gets here: one atomic per warp
+        const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, counted);
+        if ((threadIdx.x & 31) == 0 && w) atomicAdd(a.line_count, (unsigned long long)w);
     }
 }
 
 } // namespace
 
-void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
+template <bool COUNT>
+static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
     const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256;
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<COUNT>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
     {
         cudaGetLastError();
         per_sm = 1;
@@ -162,9 +189,16 @@ void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
     const uint64_t blocks_needed = (own + (uint64_t)RX_SEG * RX_THREADS - 1) / ((uint64_t)RX_SEG * RX_THREADS);
     const uint64_t resident = (uint64_t)sm_count * per_sm;
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
-    trace("regex: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", grid, RX_THREADS, per_sm, smem);
-    k_regex_lines<<<grid, RX_THREADS, smem, s>>>(a);
+    trace("regex%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", COUNT ? " count" : "", grid, RX_THREADS, per_sm,
+          smem);
+    k_regex_lines<COUNT><<<grid, RX_THREADS, smem, s>>>(a);
     count_launch();
+}
+
+void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
+{
+    if (a.line_count) launch_regex_t<true>(a, sm_count, s);
+    else launch_regex_t<false>(a, sm_count, s);
 }
 
 } // namespace kb
