@@ -139,7 +139,8 @@ uint64_t krep_b200_neon_search(const search_params_t *, const char *, size_t, ma
 /* -E: regex_search (krep.c:1389).  The GPU flags every line the regex can match in (a byte automaton built from the
  * regex string krep compiles, krep.c:2081-2145, read as a C-locale POSIX ERE under REG_NEWLINE); glibc's regexec on
  * params->compiled_regex (a const regex_t *) then runs on the flagged lines only, clipped to each run of consecutive
- * flagged lines.  Count, offsets, -w / -c / -m and every glibc detail are regexec's own.  Only for patterns that
+ * flagged lines.  Count, offsets, -w / -c / -m and every glibc detail are regexec's own (or, on the two paths below,
+ * computed on the GPU and bit for bit the same).  Only for patterns that
  * krep_b200_select_search_algorithm accepts; any other pattern makes this entry fail (count 0, krep_b200_last_error).
  * Accepted: literals and escaped punctuation, '.', bracket expressions with ranges, negation and the classes alpha,
  * digit, alnum, upper, lower, blank, punct, print, graph, xdigit; ^ $ ( ) | * + ? {m} {m,} {m,n} {,n} (counts <= 255);
@@ -149,6 +150,12 @@ uint64_t krep_b200_neon_search(const search_params_t *, const char *, size_t, ma
  * counted in the scan, and regexec sees only the lines it cannot decide (a line longer than the scan's reach, and the
  * text's last line).  The count is the same; KREP_B200_NO_FUSED_COUNT=1 turns this off
  * (krep_b200_regex_count_mode tells which path a call takes).
+ * Positions and -co (track_positions without count_lines_mode), without -w, on such a pattern compute their match
+ * offsets on the GPU when the pattern's anchored match automaton fits the scan's shared memory next to the line
+ * automaton: every line the scan decides is walked again there, leftmost-longest, as the reference's loop walks it,
+ * and regexec sees only the lines it cannot decide (those above, and a line whose walk runs over a step budget of a
+ * few automaton steps per byte).  Count, positions and their order are the same; KREP_B200_NO_DEVICE_MATCHES=1 turns
+ * this off (krep_b200_regex_match_mode tells which path a call takes).
  * Refused (the pattern stays with the host's regex_search): back-references, \` \', \s \S \W, [[:space:]],
  * [[:cntrl:]], collating elements, any character set that holds '\n' or a newline in the pattern, non-ASCII pattern
  * bytes, unknown escapes, a process running in a multibyte locale (krep itself never calls setlocale), and automata
@@ -360,14 +367,25 @@ uint64_t krep_b200_replay(int algo, const search_params_t *params, bool only_mat
 int64_t krep_b200_regex_filter_host(const search_params_t *params, const char *text, size_t n, uint64_t *line_starts,
                                     uint64_t cap, int *widened);
 
-/* Test hook: which path a -E call with params takes — 1 when it is a -c call counted on the device (see
- * krep_b200_regex_search), 0 when its lines go through regexec, -1 when the pattern is refused. */
+/* Test hook: which path a -E -c call with params takes — 1 when it is a -c call counted on the device (see
+ * krep_b200_regex_search), 0 when its lines go through regexec (every call that is not such a -c call), -1 when the
+ * pattern is refused. */
 int krep_b200_regex_count_mode(const search_params_t *params);
 /* Test hook, host only: the fused -E -c on the CPU — the line automaton decides every line it can within `reach` bytes
  * of the line's start (UINT64_MAX: no bound), and the lines it leaves uncertain (out of reach, or holding the text's
  * last byte) go to regexec as in krep_b200_regex_search.  Returns the count, or -1 when the pattern is refused or a
  * -c call with params would not be counted on the device whatever KREP_B200_NO_FUSED_COUNT says. */
 int64_t krep_b200_regex_count_host(const search_params_t *params, const char *text, size_t n, uint64_t reach);
+/* Test hook: where a -E positions or -co call with params gets its offsets — 1 when the device computes them (see
+ * krep_b200_regex_search), 0 when they come from regexec, -1 when the pattern is refused. */
+int krep_b200_regex_match_mode(const search_params_t *params);
+/* Test hook, host only: device offsets on the CPU — the line automaton decides every line it can within `reach` bytes
+ * of the line's start (UINT64_MAX: no bound), the match automaton enumerates the matches of each line decided MATCHED
+ * within the same step budget as the scan, and the lines left uncertain go to regexec as in krep_b200_regex_search.
+ * Fills res (may be NULL) and returns the count, or -1 when the pattern is refused or a call with params would not
+ * compute its offsets on the device whatever KREP_B200_NO_DEVICE_MATCHES says. */
+int64_t krep_b200_regex_matches_host(const search_params_t *params, const char *text, size_t n, uint64_t reach,
+                                     match_result_t *res);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

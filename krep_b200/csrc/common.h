@@ -65,6 +65,21 @@ struct LitDevParams
 static constexpr uint32_t REGEX_TABLE_BYTES = 32768; // transition table budget: shared memory of k_regex_lines
 static constexpr uint32_t REGEX_MAX_STATES = 4096;
 static constexpr uint32_t REGEX_HALO = 4096; // a line may run this far past its thread's segment before it is flagged unverified
+static constexpr uint32_t REGEX_SEG = 256;   // bytes of owned range per thread of k_regex_lines
+
+// Match mode of k_regex_lines (offsets on the device, DESIGN §12.2): one key per match of a line the device decides, one
+// per line it leaves to regexec.  Ascending key order is the reference's emission order; a line's uncertain key sorts
+// before any match key in it.
+//   match key     : (global_start << 16) | (len << 3) | 1    (len <= REGEX_SEG + REGEX_HALO < 2^13)
+//   uncertain key : global_line_start << 16
+static constexpr int REGEX_MATCH_SHIFT = 16;
+static constexpr uint64_t REGEX_MATCH_MAX_OFFSET = 1ull << 48;
+// The anchored match automaton shares the kernel's default dynamic shared memory with the line table and the class map.
+static constexpr uint32_t REGEX_SMEM_BYTES = 48 * 1024;
+// Enumeration budget of one line in match mode: automaton steps (plus one per start position tried) before the line is
+// left to regexec.  Keeps patterns such as [a-c]*d on long a-c runs linear.
+static constexpr uint32_t REGEX_MATCH_STEPS_PER_BYTE = 8;
+static constexpr uint32_t REGEX_MATCH_STEPS_BASE = 256;
 
 struct RegexDfa
 {
@@ -74,13 +89,27 @@ struct RegexDfa
     std::vector<uint16_t> trans;
     bool widened = false; // the automaton accepts more than the regex (word assertions, -i brackets)
     bool count_exact = false; // its per-line answer is glibc's: -c may be counted on the device (DESIGN §12.1)
+    // offsets_exact: match offsets may be computed on the device (DESIGN §12.2).  Then `match` holds the anchored match
+    // automaton over the same byte classes: row 0 is DEAD, entries are row offsets (next = match[row + cls[byte]]), and
+    // the '\n' column holds the row's accept bits instead of a transition: 1 = a match ends here, 2 = a match ends here
+    // if the line ends here (the '$' before '\n').  match_bol starts a match at the line's first byte, match_mid anywhere
+    // else.
+    bool offsets_exact = false;
+    std::vector<uint16_t> match;
+    uint32_t match_bol = 0, match_mid = 0;
 };
+static constexpr uint16_t RX_ACC = 1, RX_ACC_EOL = 2;
+// Padded size in 16-bit words of the table image the kernel copies to shared memory: line table, class map, match table.
+__host__ __device__ inline uint32_t regex_tab_words(uint32_t ntrans) { return (ntrans + 7) & ~7u; }
 bool regex_source(const search_params_t *P, std::string *out); // the string krep compiles (krep.c:2081-2145)
 int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why); // 0, or -1 = refused (*why)
 void regex_lines_host(const RegexDfa &D, const char *text, size_t n, std::vector<uint64_t> *line_starts);
 // The count mode of k_regex_lines on the host, every line walked at most `reach` bytes: returns the lines decided
 // MATCHED and stores the uncertain line starts (live at the bound, or holding the text's last byte) in *uncertain.
 uint64_t regex_count_lines_host(const RegexDfa &D, const char *text, size_t n, uint64_t reach, std::vector<uint64_t> *uncertain);
+// The match mode of k_regex_lines on the host (offsets_exact plans), every line walked at most `reach` bytes: stores the
+// match-mode keys (see REGEX_MATCH_SHIFT) in ascending order in *keys.
+void regex_matches_host(const RegexDfa &D, const char *text, size_t n, uint64_t reach, std::vector<uint64_t> *keys);
 
 struct RegexLaunch
 {
@@ -93,6 +122,8 @@ struct RegexLaunch
     uint64_t cap;
     unsigned long long *counter;
     unsigned long long *line_count; // count mode (-c): lines decided MATCHED on the device; nullptr = filter mode
+    // match mode (offsets on the device) when set: the match table follows the class map in `trans`
+    uint32_t matches, nmtrans, match_bol, match_mid;
 };
 
 struct AcDevTables;  // scan_multi.cu: one device's copy of a pattern set's tables
@@ -164,8 +195,9 @@ static constexpr uint64_t LB_OUTSIDE_SHARD = ~0ull - 2; // the line continues in
 
 // Launch one shard scan on `stream` of the device context; appends to that device's key list (no counter reset).
 // regex_lines (regex plans only): run k_regex_lines in count mode, adding the lines it decides MATCHED there.
+// regex_matches (offsets_exact regex plans, with want_positions): run it in match mode (match and uncertain-line keys).
 int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0,
-                unsigned long long *regex_lines = nullptr);
+                unsigned long long *regex_lines = nullptr, bool regex_matches = false);
 // literal kernels (scan_literal.cu)
 void launch_literal(const Plan *plan, const LitDevParams &p, int sm_count, cudaStream_t s);
 // multi kernels (scan_multi.cu)
@@ -197,11 +229,16 @@ struct Replay
     size_t text_len;
     uint64_t base; // global offset subtracted from key offsets
     const uint64_t *bounds = nullptr; // resolved line bounds, 2 per key (device-side -c): used when text is null
+    // replay_regex: the text from `stop` on (a line start below text_len) belongs to another decider — no regexec call
+    // reaches past it, and a match found there ends the replay (SIZE_MAX: the whole text is the replay's)
+    size_t stop = SIZE_MAX;
 };
 uint64_t replay_literal(int algo, const search_params_t *P, bool only_matching, uint32_t m,
                         const Replay &r, match_result_t *res);
 uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *res);
 uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res); // needs r.text
+// Offsets on the device (match-mode keys, ascending): match keys become positions, uncertain lines go to replay_regex.
+uint64_t replay_regex_matches(const search_params_t *P, const Replay &r, match_result_t *res);
 bool result_push(match_result_t *r, size_t s, size_t e);
 
 // C-locale helpers shared by host code (krep.c:125-134, krep.h:298-301)

@@ -397,11 +397,14 @@ const PlanDev *plan_on_device(const Plan *plan, DevCtx &C)
     }
     else if (plan->is_regex)
     {
-        // transition table, padded to 16 bytes, then the class map: k_regex_lines copies both to shared memory as vectors
+        // transition table, padded to 16 bytes, then the class map, then the match table of an offsets_exact plan (padded
+        // too): k_regex_lines copies what its mode reads to shared memory as vectors
         const RegexDfa &D = *plan->rx;
-        std::vector<uint16_t> img(((D.trans.size() + 7) & ~(size_t)7) + 128, 0);
+        const size_t tw = regex_tab_words((uint32_t)D.trans.size());
+        std::vector<uint16_t> img(tw + 128 + regex_tab_words((uint32_t)D.match.size()), 0);
         std::copy(D.trans.begin(), D.trans.end(), img.begin());
-        memcpy(img.data() + img.size() - 128, D.cls, 256);
+        memcpy(img.data() + tw, D.cls, 256);
+        std::copy(D.match.begin(), D.match.end(), img.begin() + tw + 128);
         if (cudaMalloc(&pd.d_regex, img.size() * 2) != cudaSuccess ||
             cudaMemcpy(pd.d_regex, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess)
         {
@@ -579,7 +582,7 @@ Plan *plan_build(const search_params_t *P, int algo, bool only_matching)
 // shard scan
 // ---------------------------------------------------------------------------------------------
 int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot,
-                unsigned long long *regex_lines)
+                unsigned long long *regex_lines, bool regex_matches)
 {
     if (((uintptr_t)sh->d_text & 15) != 0)
     {
@@ -591,6 +594,17 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
     uint64_t own_end = sh->own_end < sh->avail_len ? sh->own_end : sh->avail_len;
     if (plan->is_regex)
     {
+        if (regex_matches && (!plan->rx->offsets_exact || !want_positions))
+        {
+            set_error(-3, "regex match mode needs an offsets_exact plan and the occurrence list");
+            return -3;
+        }
+        // match keys pack (global start << 16): 48 bits of offset
+        if (regex_matches && sh->global_offset + sh->avail_len >= REGEX_MATCH_MAX_OFFSET)
+        {
+            set_error(-3, "regex match offsets must stay below 2^48 bytes of global offset (key layout, csrc/common.h)");
+            return -3;
+        }
         RegexLaunch a;
         a.text = (const uint8_t *)sh->d_text;
         a.avail_len = sh->avail_len;
@@ -608,6 +622,10 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.cap = want_positions ? E.key_cap : 0;
         a.counter = slot_counter(E, slot);
         a.line_count = regex_lines;
+        a.matches = regex_matches ? 1u : 0u;
+        a.nmtrans = (uint32_t)plan->rx->match.size();
+        a.match_bol = plan->rx->match_bol;
+        a.match_mid = plan->rx->match_mid;
         launch_regex(a, E.sm_count, stream);
         return 0;
     }
@@ -798,9 +816,9 @@ static int bits_for(uint64_t v)
     return b;
 }
 
-int key_end_bit(const Plan *plan, uint64_t max_offset)
+int key_end_bit(const Plan *plan, uint64_t max_offset, bool regex_matches)
 {
-    const int shift = plan->is_ac ? AC_END_SHIFT : LIT_TAG_BITS;
+    const int shift = plan->is_ac ? AC_END_SHIFT : regex_matches ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
     int b = bits_for(max_offset) + shift;
     return b > 64 ? 64 : b;
 }

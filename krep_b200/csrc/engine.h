@@ -120,7 +120,7 @@ int finish_scan(DevCtx &C, int slot, int want_sort, cudaStream_t stream); // k_f
 int ensure_keys(DevCtx &C, uint64_t cap);
 int reset_counter(DevCtx &C, int slot, cudaStream_t stream);
 int sort_keys(DevCtx &C, int slot, uint64_t n, int end_bit, cudaStream_t stream, const uint64_t **sorted);
-int key_end_bit(const Plan *plan, uint64_t max_offset);
+int key_end_bit(const Plan *plan, uint64_t max_offset, bool regex_matches = false); // regex_matches: match-mode keys
 int fetch_keys(DevCtx &C, const ScanOut &so, const uint64_t **h); // sorted keys on the host (no copy when they came back packed)
 void add_kernel_ms(float ms);
 void reset_kernel_ms();

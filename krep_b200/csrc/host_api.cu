@@ -310,6 +310,7 @@ struct RangeJob
     std::vector<uint64_t> line_recs; // (lines, flags) per chunk, text order
     bool regex_count = false; // fused -E -c: every chunk adds its device-decided matching lines and leaves its uncertain keys
     uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
+    bool regex_matches = false; // -E offsets on the device: match keys and uncertain-line keys (REGEX_MATCH_SHIFT layout)
     // results
     int rc = 0;
     ScanOut so;
@@ -375,7 +376,8 @@ static int stream_range(RangeJob &J)
             cudaEvent_t a = pool_event(E, 2 * c), b = pool_event(E, 2 * c + 1);
             CKH(cudaEventRecord(a, E.scan_stream));
             int rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
-                                   : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines);
+                                   : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines,
+                                                 J.regex_matches);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
             CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
@@ -415,7 +417,7 @@ static int stream_range(RangeJob &J)
                 J.so.h_sorted = E.h_pack[slot] + 1;
                 return 0;
             }
-            return sort_keys(E, slot, cnt, key_end_bit(plan, n), E.scan_stream, &J.so.d_keys);
+            return sort_keys(E, slot, cnt, key_end_bit(plan, n, J.regex_matches), E.scan_stream, &J.so.d_keys);
         }
         // list overflowed: grow it and stage the range again (the ring holds only the last chunks)
         J.so.overflow = 1;
@@ -466,8 +468,10 @@ struct HostScan
 };
 
 // count_lines: the fused -c of the plan — a line record per chunk for literals; for regex plans a device line count per
-// range next to the keys of the uncertain lines (want_positions must then be set).
-static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want_positions, HostScan *hs, bool count_lines = false)
+// range next to the keys of the uncertain lines (want_positions must then be set).  regex_matches: -E offsets on the
+// device (offsets_exact regex plans, want_positions set): the keys are match keys and uncertain-line keys.
+static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want_positions, HostScan *hs, bool count_lines = false,
+                          bool regex_matches = false)
 {
     const bool pinned = is_pinned(text);
     const size_t chunk = pinned ? env_mb("KREP_B200_CHUNK_MB", 256) : env_mb("KREP_B200_STAGE_MB", 32);
@@ -500,6 +504,7 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.pinned = pinned;
         J.count_lines = count_lines && !plan->is_regex;
         J.regex_count = count_lines && plan->is_regex;
+        J.regex_matches = regex_matches;
     }
     trace("search: %zu bytes (%s host memory), %zu device(s), %zu range(s), chunk %zu MiB", n, pinned ? "pinned" : "pageable", D, R,
           chunk >> 20);
@@ -796,10 +801,25 @@ static uint64_t regex_count_total(const search_params_t *P, uint64_t device_line
     return std::min<uint64_t>(device_lines + replay_regex(P, uncertain, nullptr), P->max_count);
 }
 
+// Can a -E call with these params compute its match offsets on the device?  Positions or -co (track_positions without
+// count_lines_mode), no -w, on a plan whose match automaton is exact and fits (offsets_exact).
+// KREP_B200_NO_DEVICE_MATCHES is not looked at here.
+static bool regex_matches_exact(const search_params_t *P, const Plan *plan)
+{
+    return P->track_positions && !P->count_lines_mode && !P->whole_word && plan->rx->offsets_exact;
+}
+
+static bool regex_matches_device(const search_params_t *P, const Plan *plan)
+{
+    return regex_matches_exact(P, plan) && !getenv("KREP_B200_NO_DEVICE_MATCHES");
+}
+
 // -E (regex_search, krep.c:1389): the device flags the lines the regex can match in (k_regex_lines), glibc's regexec
 // on the caller's regex_t confirms them and computes every offset (replay_regex).  A -c call on a count_exact plan
-// counts the lines the device can decide there and leaves glibc only the uncertain ones (regex_count_total).  The empty
-// text is answered on the host, as the reference does, without a launch.
+// counts the lines the device can decide there and leaves glibc only the uncertain ones (regex_count_total).  A
+// positions or -co call on an offsets_exact plan takes the offsets of the lines the device decides from the device and
+// leaves glibc only the uncertain ones (replay_regex_matches, DESIGN §12.2).  The empty text is answered on the host,
+// as the reference does, without a launch.
 static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, match_result_t *res)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
@@ -825,10 +845,17 @@ static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, 
         return 0;
     }
     const bool fused = regex_count_fused(P, plan);
+    const bool matches = !fused && regex_matches_device(P, plan);
     HostScan hs;
-    if (stage_and_scan(plan, text, n, 1, &hs, fused) != 0) return 0;
+    if (stage_and_scan(plan, text, n, 1, &hs, fused, matches) != 0) return 0;
     r.keys = hs.keys;
     r.n = (size_t)hs.nkeys;
+    if (matches)
+    {
+        const uint64_t ret = replay_regex_matches(P, r, res);
+        trace("search: regex offsets on the device: %llu keys (%llu)", (unsigned long long)hs.nkeys, (unsigned long long)ret);
+        return ret;
+    }
     if (fused)
     {
         const uint64_t ret = regex_count_total(P, hs.regex_lines, r);
@@ -1508,6 +1535,30 @@ int64_t krep_b200_regex_count_host(const search_params_t *P, const char *text, s
     const uint64_t device_lines = regex_count_lines_host(*pl->rx, text, n, reach, &keys);
     for (uint64_t &k : keys) k <<= LIT_TAG_BITS;
     return (int64_t)regex_count_total(P, device_lines, Replay{keys.data(), keys.size(), text, n, 0});
+}
+
+// ---- test hooks: -E offsets, decided and run on the host ----
+int krep_b200_regex_match_mode(const search_params_t *P)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl) return -1;
+    return regex_matches_device(P, pl) ? 1 : 0;
+}
+
+int64_t krep_b200_regex_matches_host(const search_params_t *P, const char *text, size_t n, uint64_t reach, match_result_t *res)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl || !regex_matches_exact(P, pl)) return -1;
+    if (P->max_count == 0 || !P->compiled_regex) return 0; // run_regex's early returns
+    if (n == 0) return (int64_t)replay_regex(P, Replay{nullptr, 0, text, 0, 0}, res);
+    if (!text) return 0;
+    std::vector<uint64_t> keys;
+    regex_matches_host(*pl->rx, text, n, reach, &keys);
+    return (int64_t)replay_regex_matches(P, Replay{keys.data(), keys.size(), text, n, 0}, res);
 }
 
 } // extern "C"

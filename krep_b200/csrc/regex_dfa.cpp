@@ -448,6 +448,77 @@ void closure(const Nfa &N, std::vector<int> seed, bool at_bol, bool at_eol, std:
     std::sort(out->begin(), out->end());
 }
 
+// The anchored match automaton of an exact plan (DESIGN §12.2): the subset construction of R itself — no restart
+// closure, so a walk from a start position reads the matches that begin there — over the byte classes of the line
+// table.  Two start states: at the line's first byte (BOL edges followed) and anywhere else (not followed).  State 0 is
+// DEAD.  Returns false when the table would not fit `budget_entries`: the plan then keeps its offsets on regexec.
+bool build_match_automaton(const Nfa &N, int start, const uint8_t *cls, int nc, const std::vector<int> &rep,
+                           size_t budget_entries, RegexDfa *D)
+{
+    const int nl = cls['\n'];
+    std::vector<std::vector<int>> sets(1); // [0] = DEAD (the empty set)
+    std::vector<char> is_bol(1, 0);
+    std::map<std::pair<std::vector<int>, int>, int> index; // (set, bol | matched << 1)
+    index.emplace(std::make_pair(std::vector<int>(), 0), 0);
+    std::vector<uint16_t> acc(1, 0);
+    auto intern = [&](std::vector<int> set, bool bol, bool matched) -> int {
+        auto key = std::make_pair(set, (bol ? 1 : 0) | (matched ? 2 : 0));
+        auto it = index.find(key);
+        if (it != index.end()) return it->second;
+        sets.push_back(std::move(set));
+        is_bol.push_back(bol ? 1 : 0);
+        acc.push_back(matched ? RX_ACC : 0);
+        index.emplace(key, (int)sets.size() - 1);
+        return (int)sets.size() - 1;
+    };
+    std::vector<int> s0;
+    bool m0 = false;
+    closure(N, {start}, true, false, &s0, &m0);
+    const int bol_state = intern(s0, true, m0);
+    closure(N, {start}, false, false, &s0, &m0);
+    const int mid_state = intern(s0, false, m0);
+    std::vector<std::vector<int>> next(1, std::vector<int>(nc, 0));
+    for (size_t s = 1; s < sets.size(); s++)
+    {
+        if (sets.size() * (size_t)nc > budget_entries) return false;
+        // accepts if the line ends here: a match that ends here anyway, or one through EOL edges (the set keeps the EOL
+        // states; BOL edges are followed at the line start)
+        if (acc[s] & RX_ACC) acc[s] |= RX_ACC_EOL;
+        else
+        {
+            std::vector<int> seed = sets[s], tmp;
+            if (is_bol[s]) seed.push_back(start);
+            bool a = false;
+            closure(N, seed, is_bol[s], true, &tmp, &a);
+            if (a) acc[s] |= RX_ACC_EOL;
+        }
+        std::vector<int> row(nc, 0);
+        for (int c = 0; c < nc; c++)
+        {
+            if (c == nl) continue; // holds the accept bits
+            const int b = rep[c];
+            std::vector<int> moved;
+            for (int x : sets[s])
+                if (N.st[x].kind == NState::CHAR && N.sets[N.st[x].set][b]) moved.push_back(N.st[x].out);
+            if (moved.empty()) continue;
+            std::vector<int> cl;
+            bool mt = false;
+            closure(N, moved, false, false, &cl, &mt);
+            row[c] = intern(cl, false, mt);
+        }
+        next.push_back(row);
+    }
+    const size_t S = sets.size();
+    if (S * (size_t)nc > budget_entries) return false;
+    D->match.assign(S * nc, 0);
+    for (size_t s = 0; s < S; s++)
+        for (int c = 0; c < nc; c++)
+            D->match[s * nc + c] = c == nl ? acc[s] : (uint16_t)(next[s][c] * nc);
+    D->match_bol = (uint32_t)(bol_state * nc);
+    D->match_mid = (uint32_t)(mid_state * nc);
+    return true;
+}
+
 } // namespace
 
 // The regular expression krep hands to regcomp (krep.c:2081-2145 and 2539-2600): patterns are read as C strings.
@@ -619,6 +690,16 @@ int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *w
         }
     D->widened = ps.widened || N.widened;
     D->count_exact = !D->widened;
+    // offsets on the device: the plans whose per-line answer is exact, when the match automaton fits the shared memory
+    // left next to the line table and the class map
+    D->offsets_exact = false;
+    if (D->count_exact)
+    {
+        const size_t used = (size_t)regex_tab_words((uint32_t)D->trans.size()) * 2 + 256;
+        const size_t budget = used < REGEX_SMEM_BYTES ? (REGEX_SMEM_BYTES - used) / 2 : 0;
+        D->offsets_exact = build_match_automaton(N, start, cls, nc, rep, budget & ~(size_t)7, D);
+        if (!D->offsets_exact) D->match.clear();
+    }
     return 0;
 }
 
@@ -666,6 +747,62 @@ uint64_t regex_count_lines_host(const RegexDfa &D, const char *t, size_t n, uint
         p = (size_t)((const char *)nl - t) + 1;
     }
     return counted;
+}
+
+// The match mode of k_regex_lines (scan_regex.cu): the line walk of the count mode, then for a line decided MATCHED the
+// reference's loop restated inside the line [p, q] (q = its '\n'): from cur, the leftmost start s with a match and its
+// longest end e, emitted; cur = e, or s + 1 after an empty match; until cur passes q.  '^' holds only at s == p, '$'
+// only at q.  A line whose enumeration runs over its step budget leaves an uncertain key behind the match keys it
+// already emitted (the host drops those).
+void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t reach, std::vector<uint64_t> *keys)
+{
+    keys->clear();
+    const uint32_t dead = D.nclasses, nl = D.nl_class;
+    const uint16_t *M = D.match.data();
+    size_t p = 0;
+    while (p < n)
+    {
+        const size_t limit = reach < n - p ? p + (size_t)reach : n;
+        uint32_t row = D.start;
+        size_t q = p;
+        for (; q < limit && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
+        if (row > dead && q < limit) row = D.trans[row + nl];
+        if (row <= dead)
+            while (q < limit && t[q] != '\n') q++;
+        if (q >= limit || q + 1 == n) keys->push_back((uint64_t)p << REGEX_MATCH_SHIFT);
+        else if (row == 0)
+        {
+            const uint64_t budget = (uint64_t)REGEX_MATCH_STEPS_PER_BYTE * (q - p) + REGEX_MATCH_STEPS_BASE;
+            uint64_t steps = 0;
+            size_t cur = p;
+            while (cur <= q && steps <= budget)
+            {
+                size_t s = cur, e = 0;
+                bool found = false;
+                for (; s <= q && steps <= budget; s++)
+                {
+                    uint32_t r = s == p ? D.match_bol : D.match_mid;
+                    steps++;
+                    if (M[r + nl] & (s == q ? RX_ACC_EOL : RX_ACC)) found = true, e = s;
+                    for (size_t x = s; x < q && r != 0;)
+                    {
+                        r = M[r + D.cls[(uint8_t)t[x++]]];
+                        steps++;
+                        if (M[r + nl] & (x == q ? RX_ACC_EOL : RX_ACC)) found = true, e = x;
+                    }
+                    if (found) break;
+                }
+                if (!found) break;
+                keys->push_back(((uint64_t)s << REGEX_MATCH_SHIFT) | ((uint64_t)(e - s) << LIT_TAG_BITS) | 1);
+                cur = e == s ? s + 1 : e;
+            }
+            if (steps > budget) keys->push_back((uint64_t)p << REGEX_MATCH_SHIFT);
+        }
+        const void *nlp = q < n ? memchr(t + q, '\n', n - q) : nullptr;
+        if (!nlp) break;
+        p = (size_t)((const char *)nlp - t) + 1;
+    }
+    std::sort(keys->begin(), keys->end());
 }
 
 } // namespace kb

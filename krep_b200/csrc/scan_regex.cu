@@ -15,7 +15,9 @@
 //     unverified: always safe, glibc then looks at it on the host;
 //   * the text is read as aligned 16-byte vectors held in registers (one LDG.128 per 16 bytes of a thread's walk);
 //   * in count mode (fused -E -c) the same walk counts the lines it decides MATCHED (one atomic per warp) and emits
-//     keys for the uncertain lines only.
+//     keys for the uncertain lines only;
+//   * in match mode (offsets on the device) the same walk decides the lines, and each line decided MATCHED is walked
+//     again with the anchored match automaton to emit one key per match, in the reference's order (DESIGN §12.2).
 //
 // Work per byte: one class lookup and one transition lookup in shared memory.
 #include <cooperative_groups.h>
@@ -29,7 +31,7 @@ namespace kb {
 namespace {
 
 constexpr int RX_THREADS = 256;
-constexpr uint32_t RX_SEG = 256; // bytes of owned range per thread
+constexpr uint32_t RX_SEG = REGEX_SEG; // bytes of owned range per thread
 
 // The aligned 16 bytes around the last position read, in registers.
 struct Window
@@ -92,28 +94,50 @@ __device__ __forceinline__ uint64_t next_newline(Window &W, uint64_t q, uint64_t
     return end;
 }
 
-// COUNT = false: the filter (one key per flagged line).  COUNT = true: the fused -c of plans whose per-line answer is
-// exact (RegexDfa::count_exact).  A line the walk decides (MATCHED or DEAD, or its '\n' read through the '\n' column)
-// is settled on the device, and a MATCHED one is counted; only the uncertain lines leave as keys: a line whose '\n' lies
+// Match mode: reserve one slot of the occurrence list per calling thread, one atomic per coalesced group, and store the
+// key there.
+__device__ __forceinline__ void emit_key(const RegexLaunch &a, uint64_t key)
+{
+    cg::coalesced_group g = cg::coalesced_threads();
+    unsigned long long base = 0;
+    if (g.thread_rank() == 0) base = atomicAdd(a.counter, (unsigned long long)g.size());
+    base = g.shfl(base, 0) + g.thread_rank();
+    if (base < a.cap) a.out[base] = key;
+}
+
+enum RxMode : int
+{
+    RX_FILTER = 0, // one key per flagged line
+    RX_COUNT = 1,  // fused -c: lines decided MATCHED are counted, uncertain lines leave keys
+    RX_MATCH = 2,  // offsets: one key per match of a line decided MATCHED, uncertain lines leave keys
+};
+
+// RX_FILTER: the filter (one key per flagged line).  RX_COUNT: the fused -c of plans whose per-line answer is exact
+// (RegexDfa::count_exact).  A line the walk decides (MATCHED or DEAD, or its '\n' read through the '\n' column) is
+// settled on the device, and a MATCHED one is counted; only the uncertain lines leave as keys: a line whose '\n' lies
 // beyond the walk's limit, and the line that holds the text's last byte (decided or not, so that both end-of-text
-// quirks of the reference stay with glibc: DESIGN §12.1).
-template <bool COUNT>
+// quirks of the reference stay with glibc: DESIGN §12.1).  RX_MATCH (RegexDfa::offsets_exact): the same uncertain
+// lines leave keys (REGEX_MATCH_SHIFT layout); a line decided MATCHED is enumerated with the anchored match automaton
+// (DESIGN §12.2) within a step budget, and a line over its budget leaves an uncertain key as well.
+template <int MODE>
 __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constant__ RegexLaunch a)
 {
     extern __shared__ uint4 s_raw[];
     uint16_t *s_tab = reinterpret_cast<uint16_t *>(s_raw);
     const uint32_t tab_words = (a.ntrans + 7) & ~7u; // the class map follows the table, 16-byte aligned
-    const uint32_t nvec = (tab_words * 2 + 256) / 16;
+    // match mode: the match table follows the class map
+    const uint32_t nvec = (tab_words * 2 + 256 + (MODE == RX_MATCH ? regex_tab_words(a.nmtrans) * 2 : 0u)) / 16;
     const uint4 *src = reinterpret_cast<const uint4 *>(a.trans);
     for (uint32_t i = threadIdx.x; i < nvec; i += blockDim.x) s_raw[i] = src[i];
     __syncthreads();
     const uint8_t *s_cls = reinterpret_cast<const uint8_t *>(s_tab + tab_words);
+    const uint16_t *s_mtab = s_tab + tab_words + 128;
     const uint32_t dead = a.nclasses, nl = a.nl_class;
 
     const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
     const uint64_t nseg = (own + RX_SEG - 1) / RX_SEG;
     Window W{a.text, a.avail_len, ~0ull, make_uint4(0, 0, 0, 0)};
-    uint32_t counted = 0; // COUNT: lines of this thread decided MATCHED
+    uint32_t counted = 0; // RX_COUNT: lines of this thread decided MATCHED
     for (uint64_t sg = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; sg < nseg; sg += (uint64_t)gridDim.x * blockDim.x)
     {
         const uint64_t sb = a.own_begin + sg * RX_SEG;
@@ -138,12 +162,12 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
                 q++;
             }
             bool flag;
-            if constexpr (COUNT)
+            if constexpr (MODE != RX_FILTER)
             {
                 if (row > dead && q < limit) row = s_tab[row + nl]; // the walk stopped at the line's '\n'
                 if (row <= dead) q = next_newline(W, q, limit);
                 flag = q >= limit || (q + 1 == a.avail_len && a.next_byte < 0); // '\n' out of reach, or the text's last byte
-                counted += (!flag && row == 0) ? 1u : 0u;
+                if constexpr (MODE == RX_COUNT) counted += (!flag && row == 0) ? 1u : 0u;
             }
             else
             {
@@ -151,21 +175,55 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
                 else if (q < limit || (q == a.avail_len && a.next_byte < 0)) flag = s_tab[row + nl] == 0; // end of the line
                 else flag = true;                                                        // line not seen to its end: unverified
             }
+            if constexpr (MODE == RX_MATCH)
+            {
+                if (!flag && row == 0)
+                {
+                    // the reference's loop inside the line [p, q]: from cur, the leftmost start s with a match and its
+                    // longest end e; then cur = e, or s + 1 after an empty match.  '^' holds at p only, '$' at q only.
+                    // offsets are relative to p: a decided line is at most RX_SEG + REGEX_HALO bytes long
+                    const uint32_t len = (uint32_t)(q - p);
+                    const uint32_t budget = REGEX_MATCH_STEPS_PER_BYTE * len + REGEX_MATCH_STEPS_BASE;
+                    uint32_t steps = 0, cur = 0;
+                    while (cur <= len && steps <= budget)
+                    {
+                        uint32_t s = cur, e = 0;
+                        bool found = false;
+                        for (; s <= len && steps <= budget; s++)
+                        {
+                            uint32_t r = s == 0 ? a.match_bol : a.match_mid;
+                            steps++;
+                            if (s_mtab[r + nl] & (s == len ? RX_ACC_EOL : RX_ACC)) found = true, e = s;
+                            for (uint32_t x = s; x < len && r != 0;)
+                            {
+                                r = s_mtab[r + s_cls[W.at(p + x++)]];
+                                steps++;
+                                if (s_mtab[r + nl] & (x == len ? RX_ACC_EOL : RX_ACC)) found = true, e = x;
+                            }
+                            if (found) break;
+                        }
+                        if (!found) break;
+                        emit_key(a, ((a.global_offset + p + s) << REGEX_MATCH_SHIFT) | ((uint64_t)(e - s) << LIT_TAG_BITS) | 1);
+                        cur = e == s ? s + 1 : e;
+                    }
+                    flag = steps > budget; // over budget: the whole line goes to regexec
+                }
+            }
             if (flag)
             {
                 cg::coalesced_group g = cg::coalesced_threads();
                 unsigned long long base = 0;
                 if (g.thread_rank() == 0) base = atomicAdd(a.counter, (unsigned long long)g.size());
                 base = g.shfl(base, 0) + g.thread_rank();
-                if (base < a.cap) a.out[base] = (a.global_offset + p) << LIT_TAG_BITS;
+                if (base < a.cap) a.out[base] = (a.global_offset + p) << (MODE == RX_MATCH ? REGEX_MATCH_SHIFT : LIT_TAG_BITS);
             }
-            if constexpr (!COUNT)
+            if constexpr (MODE == RX_FILTER)
                 if (row <= dead) q = next_newline(W, q, limit);
             if (q >= limit) break; // the next line starts beyond this thread's reach, hence beyond its segment
             p = q + 1;
         }
     }
-    if constexpr (COUNT)
+    if constexpr (MODE == RX_COUNT)
     {
         // every thread of the block gets here: one atomic per warp
         const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, counted);
@@ -175,12 +233,12 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
 
 } // namespace
 
-template <bool COUNT>
+template <int MODE>
 static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
-    const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256;
+    const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256 + (MODE == RX_MATCH ? (size_t)regex_tab_words(a.nmtrans) * 2 : 0);
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<COUNT>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
     {
         cudaGetLastError();
         per_sm = 1;
@@ -189,16 +247,17 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
     const uint64_t blocks_needed = (own + (uint64_t)RX_SEG * RX_THREADS - 1) / ((uint64_t)RX_SEG * RX_THREADS);
     const uint64_t resident = (uint64_t)sm_count * per_sm;
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
-    trace("regex%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", COUNT ? " count" : "", grid, RX_THREADS, per_sm,
-          smem);
-    k_regex_lines<COUNT><<<grid, RX_THREADS, smem, s>>>(a);
+    trace("regex%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory",
+          MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", grid, RX_THREADS, per_sm, smem);
+    k_regex_lines<MODE><<<grid, RX_THREADS, smem, s>>>(a);
     count_launch();
 }
 
 void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
-    if (a.line_count) launch_regex_t<true>(a, sm_count, s);
-    else launch_regex_t<false>(a, sm_count, s);
+    if (a.line_count) launch_regex_t<RX_COUNT>(a, sm_count, s);
+    else if (a.matches) launch_regex_t<RX_MATCH>(a, sm_count, s);
+    else launch_regex_t<RX_FILTER>(a, sm_count, s);
 }
 
 } // namespace kb

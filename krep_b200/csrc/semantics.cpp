@@ -619,8 +619,9 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
             if (!found)
             {
                 // no flagged line left.  A text that ends with '\n' still has an empty string after it, where the
-                // reference's search from the cursor can end with an empty match (^ or $ at the end of the text)
-                if (t[n - 1] != '\n') break;
+                // reference's search from the cursor can end with an empty match (^ or $ at the end of the text) —
+                // unless that end belongs to another decider
+                if (t[n - 1] != '\n' || r.stop < n) break;
                 s = e = n;
             }
             const size_t run_start = s;
@@ -659,6 +660,13 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
             continue;
         }
         const size_t start = cur + so, end = cur + eo;
+        if (r.stop < n && start >= run_end && run_end < n)
+        {
+            // an empty match at the clipped end: '^' after the run's last '\n'.  It lies in the next line, whose matches
+            // are not this replay's to report (the reference finds it there, from that line's start)
+            cur = run_end;
+            continue;
+        }
         if (P->whole_word && ((start > 0 && is_word_c((unsigned char)t[start - 1])) || (end < n && is_word_c((unsigned char)t[end]))))
         {
             cur = std::min(cur + so + 1, n); // krep.c:1487-1501
@@ -684,6 +692,66 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
         if (count >= max_count) break;
         const size_t next = cur + (so == eo ? so + 1 : eo);
         cur = next > n ? n : next;
+    }
+    return count;
+}
+
+// -E offsets on the device (DESIGN §12.2).  r.keys: ascending match-mode keys — a match key per match of a line the
+// device decided, an uncertain-line key per line it left to regexec (sorted before any match key inside that line,
+// which the replay skips: the device ran over its step budget there).  Walked in order with the -m limit applied in that
+// order: match keys become positions; each stretch of consecutive uncertain lines goes through replay_regex, stopped
+// at the next line the device decided (Replay::stop), its positions appended in order.  Exact because no match crosses
+// a line and, for plans without word assertions, what regexec finds in a line does not depend on where the cursor
+// entered it (at or before the line's start).
+uint64_t replay_regex_matches(const search_params_t *P, const Replay &r, match_result_t *res)
+{
+    const char *t = r.text;
+    const size_t n = r.text_len;
+    const uint64_t max_count = P->max_count;
+    auto after_line = [&](size_t s) {
+        const size_t e = line_end(t, n, s);
+        return e < n ? e + 1 : n;
+    };
+    std::vector<uint64_t> lines; // uncertain line starts, shifted as replay_regex reads them
+    uint64_t count = 0;
+    size_t i = 0;
+    while (i < r.n && count < max_count)
+    {
+        const uint64_t k = r.keys[i];
+        const size_t pos = (size_t)((k >> REGEX_MATCH_SHIFT) - r.base);
+        if (k & 1)
+        {
+            const size_t len = (size_t)((k >> LIT_TAG_BITS) & ((1u << (REGEX_MATCH_SHIFT - LIT_TAG_BITS)) - 1));
+            count++;
+            if (res) result_push(res, pos, pos + len);
+            i++;
+            continue;
+        }
+        // a stretch of uncertain lines: up to the next match key outside them
+        lines.clear();
+        size_t end = 0;
+        while (i < r.n)
+        {
+            const uint64_t u = r.keys[i];
+            const size_t s = (size_t)((u >> REGEX_MATCH_SHIFT) - r.base);
+            if (u & 1)
+            {
+                if (s < end) // a match key inside an uncertain line
+                {
+                    i++;
+                    continue;
+                }
+                break;
+            }
+            lines.push_back((uint64_t)s << LIT_TAG_BITS);
+            end = after_line(s);
+            i++;
+        }
+        search_params_t sub = *P;
+        sub.max_count = (size_t)(max_count - count);
+        Replay g{lines.data(), lines.size(), t, n, 0};
+        g.stop = end < n ? end : SIZE_MAX;
+        count += replay_regex(&sub, g, res);
     }
     return count;
 }

@@ -107,6 +107,10 @@ def load():
     L.krep_b200_regex_count_mode.restype = C.c_int
     L.krep_b200_regex_count_host.argtypes = [C.POINTER(SearchParams), C.c_void_p, C.c_size_t, C.c_uint64]
     L.krep_b200_regex_count_host.restype = C.c_int64
+    L.krep_b200_regex_match_mode.argtypes = [C.POINTER(SearchParams)]
+    L.krep_b200_regex_match_mode.restype = C.c_int
+    L.krep_b200_regex_matches_host.argtypes = [C.POINTER(SearchParams), C.c_void_p, C.c_size_t, C.c_uint64, C.POINTER(MatchResult)]
+    L.krep_b200_regex_matches_host.restype = C.c_int64
     L.krep_b200_last_kernel_ms.restype = C.c_float
     L.krep_b200_launch_count.restype = C.c_uint64
     for n in ("krep_b200_ac_key_end", "krep_b200_ac_key_start"):
