@@ -386,6 +386,14 @@ int krep_b200_regex_match_mode(const search_params_t *params);
  * compute its offsets on the device whatever KREP_B200_NO_DEVICE_MATCHES says. */
 int64_t krep_b200_regex_matches_host(const search_params_t *params, const char *text, size_t n, uint64_t reach,
                                      match_result_t *res);
+/* Test hook: one k_regex_lines scan of a resident shard in `mode` (0 = line filter, 1 = fused -c count,
+ * 2 = match offsets). The keys, sorted ascending, go to keys[0 .. min(result, cap)), in the layout of that mode
+ * (csrc/common.h). *device_lines (may be NULL) receives the count mode's counter of lines decided MATCHED (0 in the
+ * other modes). Returns the exact number of keys, or a negative error. Errors: plan not a regex plan; mode 1 on a plan
+ * that is not count_exact; mode 2 on a plan that is not offsets_exact; global_offset + avail_len >= 2^48 in mode 2.
+ * No search entry point calls it. */
+int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
+                                       uint64_t *keys, uint64_t cap, uint64_t *device_lines);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

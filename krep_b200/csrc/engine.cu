@@ -1248,6 +1248,75 @@ int krep_b200_scan_shard(const krep_b200_plan_t *plan, const krep_b200_shard_t *
     return krep_b200_scan_shard_end(ticket, out);
 }
 
+// One k_regex_lines scan in the given mode, its keys sorted and read back.  Unlike scan_end's retry, an overflow re-scan
+// keeps the mode and zeroes the line counter again, so the keys and the count are those of one complete scan.
+int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep_b200_shard_t *shard, int mode, uint64_t *keys,
+                                       uint64_t cap, uint64_t *device_lines)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    const Plan *plan = reinterpret_cast<const Plan *>(plan_);
+    if (!plan || !shard || (cap && !keys))
+    {
+        set_error(-3, "krep_b200_regex_scan_shard_raw: null argument");
+        return -3;
+    }
+    if (!plan->is_regex || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    {
+        set_error(-3, "krep_b200_regex_scan_shard_raw: mode %d is not available for this plan", mode);
+        return -3;
+    }
+    DeviceGuard guard;
+    DevCtx *Cp = ctx_of_pointer(shard->d_text);
+    if (!Cp) return -1;
+    DevCtx &E = *Cp;
+    for (int s = 0; s < SCAN_SLOTS; s++)
+        if (E.pend[s].active)
+        {
+            set_error(-3, "krep_b200_regex_scan_shard_raw: a scan is in flight on device %d", E.device);
+            return -3;
+        }
+    if (ensure_keys(E, 1) != 0 || (mode == 1 && ensure_line_out(E, 1) != 0)) return -2;
+    unsigned long long *d_lines = mode == 1 ? (unsigned long long *)E.d_line_out : nullptr;
+    const int slot = 0;
+    cudaStream_t st = E.scan_stream;
+    ++E.serial; // slot 0's lists are overwritten: a device result handed out earlier no longer passes the stale check
+    for (int attempt = 0; attempt < 3; attempt++)
+    {
+        CK(cudaStreamWaitEvent(st, E.ev_done[slot], 0));
+        if (reset_counter(E, slot, st) != 0) return -2;
+        if (d_lines) CK(cudaMemsetAsync(d_lines, 0, sizeof(unsigned long long), st));
+        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2);
+        if (rc != 0) return rc;
+        if (finish_scan(E, slot, 1, st) != 0) return -2;
+        if (d_lines) CK(cudaMemcpyAsync(E.h_line_out, d_lines, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        const uint64_t cnt = E.h_pack[slot][0];
+        if (cnt > E.key_cap)
+        {
+            if (ensure_keys(E, cnt + cnt / 8 + 1024) != 0) return -2;
+            continue;
+        }
+        const uint64_t n = cnt < cap ? cnt : cap;
+        if (cnt <= PACK_KEYS)
+        {
+            if (n) memcpy(keys, E.h_pack[slot] + 1, n * sizeof(uint64_t));
+        }
+        else
+        {
+            const uint64_t *d_sorted = nullptr;
+            rc = sort_keys(E, slot, cnt, key_end_bit(plan, shard->global_offset + shard->avail_len, mode == 2), st, &d_sorted);
+            if (rc != 0) return rc;
+            if (n) CK(cudaMemcpyAsync(keys, d_sorted, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+            CK(cudaStreamSynchronize(st));
+        }
+        if (device_lines) *device_lines = d_lines ? E.h_line_out[0] : 0;
+        return (int64_t)cnt;
+    }
+    set_error(-4, "occurrence list kept overflowing");
+    return -4;
+}
+
 int krep_b200_export_keys(const krep_b200_device_result_t *dev, void *d_dst, uint64_t max_keys, void *stream)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());

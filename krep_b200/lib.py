@@ -111,6 +111,9 @@ def load():
     L.krep_b200_regex_match_mode.restype = C.c_int
     L.krep_b200_regex_matches_host.argtypes = [C.POINTER(SearchParams), C.c_void_p, C.c_size_t, C.c_uint64, C.POINTER(MatchResult)]
     L.krep_b200_regex_matches_host.restype = C.c_int64
+    L.krep_b200_regex_scan_shard_raw.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.POINTER(C.c_uint64), C.c_uint64,
+                                                 C.POINTER(C.c_uint64)]
+    L.krep_b200_regex_scan_shard_raw.restype = C.c_int64
     L.krep_b200_last_kernel_ms.restype = C.c_float
     L.krep_b200_launch_count.restype = C.c_uint64
     for n in ("krep_b200_ac_key_end", "krep_b200_ac_key_start"):
