@@ -223,8 +223,10 @@ typedef struct krep_b200_plan krep_b200_plan_t; /* compiled pattern set, device-
  * A REGEX plan's scan emits one key per line the regex may match in,
  * (global line start << 3); lines longer than about 4 KiB past a thread's
  * 256-byte segment, or cut by the shard's end, are flagged without a verdict.
- * Such keys are confirmed only by krep_b200_replay(KREP_B200_ALGO_REGEX, ...)
- * with the host text; krep_b200_collect / _search_shards refuse regex plans. */
+ * Such keys are confirmed by krep_b200_replay(KREP_B200_ALGO_REGEX, ...) with
+ * the host text, or, for resident shards without one, by
+ * krep_b200_search_shards (krep_b200_regex_export_shard + _regex_resolve);
+ * krep_b200_collect refuses regex plans. */
 krep_b200_plan_t *krep_b200_plan_create(const search_params_t *params, int algo);
 void krep_b200_plan_destroy(krep_b200_plan_t *plan);
 /* Which device filter the plan uses (for bench/config reporting). */
@@ -336,7 +338,8 @@ uint64_t krep_b200_combine_line_counts(const krep_b200_line_count_t *recs, size_
  * Count-lines mode (-c) uses the line bounds the scan computed on the device
  * (plan created from params with count_lines_mode set, single shard: the
  * shard must not cut a line, i.e. prev_byte = next_byte = -1 or newline-aligned).
- * Returns the count the reference would return. */
+ * Returns the count the reference would return.  Regex plans are refused (error -3): a device result does not carry
+ * its shard's text, which glibc needs; use krep_b200_search_shards. */
 uint64_t krep_b200_collect(const krep_b200_plan_t *plan, const search_params_t *params,
                            const krep_b200_device_result_t *dev, match_result_t *result);
 
@@ -344,9 +347,36 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan, const search_params_t *
  * chunk loop and merge (krep.c:2851-3004) for text that already lives in HBM.  Shards on distinct devices are scanned
  * concurrently, the per-shard lists merged by key, and the policy replayed ONCE over the whole list, so overlap rules,
  * -m and the emission order are those of the reference's single-chunk run.  -c is answered by the fused line count
- * (single literals; line cuts between shards are resolved). */
+ * (single literals; line cuts between shards are resolved).
+ *
+ * Regex plans (-E): returns the count and positions krep_b200_regex_search(params, text, n, result) returns on the text
+ * the shards hold — the same path (fused -c, offsets on the device, or the line filter + regexec), the same knobs
+ * (KREP_B200_NO_FUSED_COUNT, KREP_B200_NO_DEVICE_MATCHES), the same early returns and -m / -w / -i / -o / -c behaviour —
+ * without a host copy of the text: each shard's row (krep_b200_regex_export_shard) brings back the bytes of the lines
+ * glibc must see, and krep_b200_regex_resolve answers from the rows.  The shards must tile one whole text: the first
+ * has global_offset + own_begin == 0 and prev_byte == -1, consecutive owned ranges abut, the last has next_byte == -1
+ * and own_end == avail_len; any other geometry fails with error -3.  The halo (avail_len - own_end) may be anything
+ * from 0: a smaller one only leaves more lines to glibc.  Offsets on the device keep the match keys' limit: a call that
+ * takes that path fails with error -3 when a shard ends at or beyond 2^48 bytes of global offset (set
+ * KREP_B200_NO_DEVICE_MATCHES for the filter path there). */
 uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan, const search_params_t *params,
                                  const krep_b200_shard_t *shards, uint32_t n_shards, match_result_t *result);
+
+/* -E over resident shards in two steps, so that one code path serves one process and a multi-rank gather (each rank
+ * exports its shards' rows, one variable-length gather brings them to one host, which resolves).
+ * krep_b200_regex_export_shard: one k_regex_lines scan of the shard in the mode krep_b200_regex_search would use for
+ * params, then the pack kernels: the shard's row (layout: csrc/common.h, RegexRowHeader) in engine-owned device memory
+ * of the shard's device — *d_row (may be NULL), valid until the next export on that device — and *row_bytes.  When dst
+ * is not NULL the row is also copied there (host or device memory, dst_cap bytes of room; -5 and nothing copied when
+ * the row does not fit).  Work queued on `stream` (may be NULL) is waited for first.  Returns 0 or a negative error. */
+int krep_b200_regex_export_shard(const krep_b200_plan_t *plan, const search_params_t *params, const krep_b200_shard_t *shard,
+                                 void *stream, void *dst, uint64_t dst_cap, uint64_t *row_bytes, const void **d_row);
+/* The answer of the search from the rows (host memory, text order) of shards that tile the text: what
+ * krep_b200_search_shards returns.  Host only; 0 with error -3 when the rows are not rows of one tiling. */
+uint64_t krep_b200_regex_resolve(const search_params_t *params, const void *const *rows, uint32_t n_rows, match_result_t *result);
+/* Timing of the most recent krep_b200_search_shards (regex plan) or krep_b200_regex_export_shard call on this thread,
+ * summed over its shards: device ms of the scans (with their sort) and of the pack kernels, and the row bytes. */
+void krep_b200_regex_export_stats(float *scan_ms, float *pack_ms, uint64_t *packed_bytes);
 
 /* Policy replay over a caller-supplied, ascending occurrence-key list in HOST memory (what
  * krep_b200_collect does after reading the device list back).  A multi-GPU host gathers the

@@ -111,6 +111,47 @@ uint64_t regex_count_lines_host(const RegexDfa &D, const char *text, size_t n, u
 // match-mode keys (see REGEX_MATCH_SHIFT) in ascending order in *keys.
 void regex_matches_host(const RegexDfa &D, const char *text, size_t n, uint64_t reach, std::vector<uint64_t> *keys);
 
+// A shard's -E row (krep_b200_regex_export_shard, DESIGN §12.4): what the host needs of one resident shard to finish a
+// regex search without the text.  One flat, 16-byte aligned buffer, every part padded to 16 bytes:
+//   RegexRowHeader                      128 bytes
+//   keys[nkeys]                         the shard's sorted keys, in the layout of its mode (filter / count: line start
+//                                       << LIT_TAG_BITS; match: REGEX_MATCH_SHIFT layout)
+//   segs[nseg]                          RegexRowSeg: global start, (length << 1) | cont
+//   head bytes                          head_len bytes (ROW_HEAD only)
+//   segment bytes                       one per segment, in order
+// A segment is a maximal run of consecutive lines glibc must see (filter and count mode: every key's line; match mode:
+// the uncertain lines, keys with low bit 0), from its first line start up to and including its last line's '\n'.  The
+// '\n' is searched up to avail_len; a segment whose last line runs past avail_len is cut there and has cont = 1 (the
+// line goes on in the next shards).  The head is the shard's own bytes from own_begin up to and including its first
+// '\n' (the whole owned range when it holds none), present when the shard starts mid-line: the resolver continues a cut
+// line with the heads of the shards that follow it, through as many shards as the line spans.
+static constexpr uint64_t REGEX_ROW_MAGIC = 0x31776f725f78726bull; // "krx_row1"
+static constexpr uint64_t ROW_HEAD = 1;  // the head is present (the shard starts mid-line)
+static constexpr uint64_t ROW_LAST = 2;  // the shard ends the text: last_byte holds the text's last byte
+static constexpr uint64_t ROW_LAST_BYTE_SHIFT = 8;
+struct RegexRowHeader
+{
+    uint64_t magic;
+    uint64_t mode;         // 0 filter, 1 count (fused -c), 2 match (offsets on the device)
+    uint64_t row_bytes;    // the whole row, a multiple of 16
+    uint64_t device_lines; // count mode: lines of the shard decided MATCHED on the device
+    uint64_t nkeys, nseg, head_len;
+    uint64_t flags;        // ROW_HEAD | ROW_LAST | last byte << ROW_LAST_BYTE_SHIFT
+    uint64_t own_begin, own_end, avail_end; // global offsets of the owned range and of the end of the readable bytes
+    uint64_t reserved[5];
+};
+static_assert(sizeof(RegexRowHeader) == 128, "row header layout");
+struct RegexRowSeg
+{
+    uint64_t start;    // global offset of the segment's first byte (a line start)
+    uint64_t len_cont; // (bytes << 1) | cont
+};
+__host__ __device__ inline uint64_t round16(uint64_t v) { return (v + 15) & ~15ull; }
+__host__ __device__ inline uint64_t regex_row_fixed_bytes(uint64_t nkeys, uint64_t nseg)
+{
+    return sizeof(RegexRowHeader) + round16(nkeys * 8 + nseg * sizeof(RegexRowSeg));
+}
+
 struct RegexLaunch
 {
     const uint8_t *text;
@@ -232,6 +273,19 @@ struct Replay
     // replay_regex: the text from `stop` on (a line start below text_len) belongs to another decider — no regexec call
     // reaches past it, and a match found there ends the replay (SIZE_MAX: the whole text is the replay's)
     size_t stop = SIZE_MAX;
+    // replay_regex over a window of the text (resident shards, DESIGN §12.4): `text` holds the bytes of global
+    // [origin, origin + window_len), whole lines starting at a line start, while text_len stays the whole text's length.
+    // window_len SIZE_MAX: `text` is the whole text.  last_byte: the text's last byte when the window does not hold it.
+    size_t origin = 0;
+    size_t window_len = SIZE_MAX;
+    int last_byte = -1;
+};
+// One window of a windowed replay: global [origin, origin + len), whole lines.
+struct RegexWindow
+{
+    size_t origin;
+    const char *bytes;
+    size_t len;
 };
 uint64_t replay_literal(int algo, const search_params_t *P, bool only_matching, uint32_t m,
                         const Replay &r, match_result_t *res);
@@ -239,6 +293,16 @@ uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *re
 uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res); // needs r.text
 // Offsets on the device (match-mode keys, ascending): match keys become positions, uncertain lines go to replay_regex.
 uint64_t replay_regex_matches(const search_params_t *P, const Replay &r, match_result_t *res);
+// The same two replays over windows of the text instead of the whole text (ascending, disjoint; every key's line lies in
+// one): window by window in order, the -m budget carried.  n: the whole text's length, last_byte its last byte.
+// replay_regex_windows takes LIT_TAG_BITS keys; at_end: also decide the empty string at n after the last window.
+uint64_t replay_regex_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w, size_t nw,
+                              size_t n, int last_byte, bool at_end, match_result_t *res);
+uint64_t replay_regex_matches_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w,
+                                      size_t nw, size_t n, int last_byte, match_result_t *res);
+// regex_rows.cpp: the answer of a -E search from the rows of the shards that tile the text (text order).  *err: 0, or
+// -3 with the error set.
+uint64_t regex_resolve_rows(const search_params_t *P, const void *const *rows, uint32_t n_rows, match_result_t *res, int *err);
 bool result_push(match_result_t *r, size_t s, size_t e);
 
 // C-locale helpers shared by host code (krep.c:125-134, krep.h:298-301)

@@ -272,6 +272,7 @@ static void ctx_destroy(DevCtx &E)
     cudaFree(E.d_line_out);
     cudaFreeHost(E.h_line_out);
     cudaFreeHost(E.h_keys);
+    regex_pack_free(E);
     for (int s = 0; s < SCAN_SLOTS; s++)
     {
         cudaFree(E.d_pack[s]);
@@ -1248,32 +1249,20 @@ int krep_b200_scan_shard(const krep_b200_plan_t *plan, const krep_b200_shard_t *
     return krep_b200_scan_shard_end(ticket, out);
 }
 
-// One k_regex_lines scan in the given mode, its keys sorted and read back.  Unlike scan_end's retry, an overflow re-scan
-// keeps the mode and zeroes the line counter again, so the keys and the count are those of one complete scan.
-int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep_b200_shard_t *shard, int mode, uint64_t *keys,
-                                       uint64_t cap, uint64_t *device_lines)
+} // extern "C"
+
+// One k_regex_lines scan of a shard in the given mode (0 filter, 1 count, 2 match) on the device's scan stream, its keys
+// sorted on the device: *d_sorted (device, *cnt keys; short lists sorted by k_finish into d_pack, longer ones by the radix
+// sort, enqueued on the stream) and the count mode's line counter.  Unlike scan_end's retry, an overflow re-scan keeps the
+// mode and zeroes the line counter again, so the keys and the count are those of one complete scan.  The lists stay valid
+// until the next scan on the device.
+int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt_out,
+                        const uint64_t **d_sorted, uint64_t *device_lines)
 {
-    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    clear_error();
-    const Plan *plan = reinterpret_cast<const Plan *>(plan_);
-    if (!plan || !shard || (cap && !keys))
-    {
-        set_error(-3, "krep_b200_regex_scan_shard_raw: null argument");
-        return -3;
-    }
-    if (!plan->is_regex || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
-    {
-        set_error(-3, "krep_b200_regex_scan_shard_raw: mode %d is not available for this plan", mode);
-        return -3;
-    }
-    DeviceGuard guard;
-    DevCtx *Cp = ctx_of_pointer(shard->d_text);
-    if (!Cp) return -1;
-    DevCtx &E = *Cp;
     for (int s = 0; s < SCAN_SLOTS; s++)
         if (E.pend[s].active)
         {
-            set_error(-3, "krep_b200_regex_scan_shard_raw: a scan is in flight on device %d", E.device);
+            set_error(-3, "%s: a scan is in flight on device %d", who, E.device);
             return -3;
         }
     if (ensure_keys(E, 1) != 0 || (mode == 1 && ensure_line_out(E, 1) != 0)) return -2;
@@ -1297,24 +1286,58 @@ int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep
             if (ensure_keys(E, cnt + cnt / 8 + 1024) != 0) return -2;
             continue;
         }
-        const uint64_t n = cnt < cap ? cnt : cap;
-        if (cnt <= PACK_KEYS)
+        *d_sorted = E.d_pack[slot] + 1;
+        if (cnt > PACK_KEYS)
         {
-            if (n) memcpy(keys, E.h_pack[slot] + 1, n * sizeof(uint64_t));
-        }
-        else
-        {
-            const uint64_t *d_sorted = nullptr;
-            rc = sort_keys(E, slot, cnt, key_end_bit(plan, shard->global_offset + shard->avail_len, mode == 2), st, &d_sorted);
+            rc = sort_keys(E, slot, cnt, key_end_bit(plan, shard->global_offset + shard->avail_len, mode == 2), st, d_sorted);
             if (rc != 0) return rc;
-            if (n) CK(cudaMemcpyAsync(keys, d_sorted, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-            CK(cudaStreamSynchronize(st));
         }
+        *cnt_out = cnt;
         if (device_lines) *device_lines = d_lines ? E.h_line_out[0] : 0;
-        return (int64_t)cnt;
+        return 0;
     }
     set_error(-4, "occurrence list kept overflowing");
     return -4;
+}
+
+extern "C" {
+
+// One k_regex_lines scan in the given mode, its keys sorted and read back.
+int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep_b200_shard_t *shard, int mode, uint64_t *keys,
+                                       uint64_t cap, uint64_t *device_lines)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    const Plan *plan = reinterpret_cast<const Plan *>(plan_);
+    if (!plan || !shard || (cap && !keys))
+    {
+        set_error(-3, "krep_b200_regex_scan_shard_raw: null argument");
+        return -3;
+    }
+    if (!plan->is_regex || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    {
+        set_error(-3, "krep_b200_regex_scan_shard_raw: mode %d is not available for this plan", mode);
+        return -3;
+    }
+    DeviceGuard guard;
+    DevCtx *Cp = ctx_of_pointer(shard->d_text);
+    if (!Cp) return -1;
+    DevCtx &E = *Cp;
+    uint64_t cnt = 0;
+    const uint64_t *d_sorted = nullptr;
+    const int rc = regex_scan_keys(E, plan, shard, mode, "krep_b200_regex_scan_shard_raw", &cnt, &d_sorted, device_lines);
+    if (rc != 0) return rc;
+    const uint64_t n = cnt < cap ? cnt : cap;
+    if (cnt <= PACK_KEYS)
+    {
+        if (n) memcpy(keys, E.h_pack[0] + 1, n * sizeof(uint64_t));
+    }
+    else if (n)
+    {
+        CK(cudaMemcpyAsync(keys, d_sorted, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, E.scan_stream));
+        CK(cudaStreamSynchronize(E.scan_stream));
+    }
+    return (int64_t)cnt;
 }
 
 int krep_b200_export_keys(const krep_b200_device_result_t *dev, void *d_dst, uint64_t max_keys, void *stream)

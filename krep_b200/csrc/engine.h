@@ -32,6 +32,8 @@ struct PendingScan
     cudaStream_t stream = nullptr;
 };
 
+struct RegexPackBufs;
+
 struct DevCtx
 {
     bool ready = false;
@@ -78,7 +80,24 @@ struct DevCtx
     uint64_t h_keys_cap = 0;
     uint8_t *h_batch = nullptr; // pinned: texts of one krep_b200_search_batch call, packed
     uint64_t h_batch_cap = 0;
+    RegexPackBufs *rx_pack = nullptr; // -E rows of resident shards (scan_regex_pack.cu)
 };
+
+// scan_regex_pack.cu — the -E row of a resident shard (layout: RegexRowHeader, csrc/common.h)
+struct RegexPackStats
+{
+    float scan_ms = 0.f, pack_ms = 0.f; // device time: the k_regex_lines scan with its sort, and the pack kernels
+    uint64_t packed_bytes = 0;          // row bytes
+};
+// One k_regex_lines scan of the shard in `mode` with its keys sorted on the device (engine.cu).
+int regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt,
+                    const uint64_t **d_sorted, uint64_t *device_lines);
+// Packs the row of the shard whose sorted keys (nkeys, in `mode`'s layout) are at d_keys into engine-owned device memory
+// on the device's scan stream, and synchronises: *d_row, *row_bytes.  The row stays valid until the next pack on the device.
+int regex_pack_row(DevCtx &E, const krep_b200_shard_t *sh, int mode, const uint64_t *d_keys, uint64_t nkeys,
+                   uint64_t device_lines, const void **d_row, uint64_t *row_bytes, float *pack_ms);
+uint8_t *regex_pack_host_buffer(DevCtx &E, uint64_t bytes); // pinned host room for a row read-back (grown as needed)
+void regex_pack_free(DevCtx &E);
 
 struct ErrState
 {

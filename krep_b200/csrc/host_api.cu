@@ -868,6 +868,109 @@ static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, 
     return ret;
 }
 
+// ---- -E on resident shards (DESIGN §12.4): a row per shard, resolved on the host ----
+static thread_local RegexPackStats t_rx_stats; // of the most recent krep_b200_search_shards / _regex_export_shard call
+
+// The k_regex_lines mode a -E call with these params takes, as in run_regex: 1 = fused -c, 2 = offsets, 0 = filter.
+static int regex_call_mode(const search_params_t *P, const Plan *plan)
+{
+    return regex_count_fused(P, plan) ? 1 : regex_matches_device(P, plan) ? 2 : 0;
+}
+
+// Scan + pack of one shard: the row is left in the engine's memory of the shard's device.
+static int regex_export(const Plan *plan, const search_params_t *P, const krep_b200_shard_t *sh, const char *who, DevCtx **ctx,
+                        const void **d_row, uint64_t *row_bytes)
+{
+    if (!plan->is_regex)
+    {
+        set_error(-3, "%s: not a regex plan", who);
+        return -3;
+    }
+    cudaPointerAttributes a;
+    DevCtx *C = (cudaPointerGetAttributes(&a, sh->d_text) == cudaSuccess && a.type == cudaMemoryTypeDevice) ? ctx_get(a.device) : ctx_primary();
+    cudaGetLastError();
+    if (!C) return -1;
+    cudaSetDevice(C->device);
+    const int mode = regex_call_mode(P, plan);
+    uint64_t cnt = 0, lines = 0;
+    const uint64_t *d_sorted = nullptr;
+    CKH(cudaEventRecord(C->ev_ca, C->scan_stream));
+    int rc = regex_scan_keys(*C, plan, sh, mode, who, &cnt, &d_sorted, &lines);
+    if (rc != 0) return rc;
+    CKH(cudaEventRecord(C->ev_cb, C->scan_stream));
+    float pack_ms = 0.f, scan_ms = 0.f;
+    rc = regex_pack_row(*C, sh, mode, d_sorted, cnt, lines, d_row, row_bytes, &pack_ms);
+    if (rc != 0) return rc;
+    cudaEventElapsedTime(&scan_ms, C->ev_ca, C->ev_cb);
+    t_rx_stats.scan_ms += scan_ms;
+    t_rx_stats.pack_ms += pack_ms;
+    t_rx_stats.packed_bytes += *row_bytes;
+    trace("regex row: mode %d, %llu keys, %llu bytes (scan %.3f ms, pack %.3f ms)", mode, (unsigned long long)cnt,
+          (unsigned long long)*row_bytes, scan_ms, pack_ms);
+    *ctx = C;
+    return 0;
+}
+
+// The shards of a -E search must tile one whole text: owned ranges that abut from offset 0 to the text's end.
+static bool regex_tiling_ok(const krep_b200_shard_t *s, uint32_t n)
+{
+    if (n == 0 || !s) return false;
+    if (s[0].global_offset + s[0].own_begin != 0 || s[0].prev_byte != -1) return false;
+    for (uint32_t i = 0; i < n; i++)
+    {
+        if (s[i].own_begin > s[i].own_end || s[i].own_end > s[i].avail_len) return false;
+        if (i && s[i - 1].global_offset + s[i - 1].own_end != s[i].global_offset + s[i].own_begin) return false;
+    }
+    return s[n - 1].next_byte == -1 && s[n - 1].own_end == s[n - 1].avail_len;
+}
+
+// krep_b200_search_shards for a regex plan: krep_b200_regex_search's answer on the text the shards tile, from one row per
+// shard (scanned and packed on the shard's device, read back in one copy) resolved by regex_resolve_rows.
+static uint64_t search_shards_regex(const Plan *plan, const search_params_t *P, const krep_b200_shard_t *shards, uint32_t n_shards,
+                                    match_result_t *res)
+{
+    t_rx_stats = RegexPackStats();
+    if (!regex_tiling_ok(shards, n_shards))
+    {
+        set_error(-3, "krep_b200_search_shards: the shards of a regex search must tile one text: the first owns from global "
+                      "offset 0 with prev_byte -1, owned ranges abut, the last has next_byte -1 and own_end == avail_len");
+        return 0;
+    }
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
+    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    const krep_b200_shard_t &last = shards[n_shards - 1];
+    if (last.global_offset + last.avail_len == 0) return replay_regex(P, Replay{nullptr, 0, nullptr, 0, 0}, res); // krep.c:1403
+    DeviceGuard guard;
+    std::vector<std::vector<uint8_t>> copies(n_shards > 1 ? n_shards : 0);
+    std::vector<const void *> rows(n_shards);
+    for (uint32_t i = 0; i < n_shards; i++)
+    {
+        DevCtx *C = nullptr;
+        const void *d_row = nullptr;
+        uint64_t bytes = 0;
+        if (regex_export(plan, P, &shards[i], "krep_b200_search_shards", &C, &d_row, &bytes) != 0) return 0;
+        uint8_t *h = regex_pack_host_buffer(*C, bytes);
+        if (!h) return 0;
+        if (cudaMemcpyAsync(h, d_row, bytes, cudaMemcpyDeviceToHost, C->scan_stream) != cudaSuccess ||
+            cudaStreamSynchronize(C->scan_stream) != cudaSuccess)
+        {
+            set_error(-2, "reading a regex row back failed (%s)", cudaGetErrorString(cudaGetLastError()));
+            return 0;
+        }
+        if (n_shards == 1) rows[i] = h; // the pinned buffer is the next row's too: keep a copy when there is one
+        else
+        {
+            copies[i].assign(h, h + bytes);
+            rows[i] = copies[i].data();
+        }
+    }
+    int err = 0;
+    const uint64_t ret = regex_resolve_rows(P, rows.data(), n_shards, res, &err);
+    trace("search_shards: regex over %u shards, %llu row bytes (%llu)", n_shards, (unsigned long long)t_rx_stats.packed_bytes,
+          (unsigned long long)ret);
+    return err ? 0 : ret;
+}
+
 // Many texts, one launch (SURVEY §8 f4: small files lose to launch and copy latency one by one).  The texts are packed
 // into one pinned buffer at 16-byte aligned offsets, separated by zero gaps longer than the longest pattern, copied and
 // scanned as ONE shard; the sorted occurrence list is then cut per text — an occurrence belongs to a text only if it
@@ -1318,12 +1421,7 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan_, const search_par
         set_error(-3, "krep_b200_search_shards: null argument");
         return 0;
     }
-    if (plan->is_regex)
-    {
-        set_error(-3, "krep_b200_search_shards: regex plans need the host text: scan the shards, merge the keys and call "
-                      "krep_b200_replay with KREP_B200_ALGO_REGEX");
-        return 0;
-    }
+    if (plan->is_regex) return search_shards_regex(plan, P, shards, n_shards, result);
     DeviceGuard guard;
     std::vector<DevCtx *> ctx(n_shards, nullptr);
     uint64_t text_len = 0;
@@ -1433,8 +1531,8 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan_, const search_params_t 
     if (!plan || !P || !dev) return 0;
     if (plan->is_regex)
     {
-        set_error(-3, "krep_b200_collect: regex plans need the host text: export the keys and call krep_b200_replay with "
-                      "KREP_B200_ALGO_REGEX");
+        set_error(-3, "krep_b200_collect: a device result does not carry its shard's text, which a regex plan needs: call "
+                      "krep_b200_search_shards (or krep_b200_regex_export_shard + krep_b200_regex_resolve)");
         return 0;
     }
     if (P->count_lines_mode && dev->stored && !dev->d_line_bounds)
@@ -1495,6 +1593,60 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan_, const search_params_t 
     }
     if (plan->is_ac) return replay_ac(P, r, result);
     return replay_literal(plan->algo, P, plan->built_only_matching, plan->m, r, result);
+}
+
+// ---- -E rows of resident shards ----
+int krep_b200_regex_export_shard(const krep_b200_plan_t *plan_, const search_params_t *P, const krep_b200_shard_t *shard, void *stream,
+                                 void *dst, uint64_t dst_cap, uint64_t *row_bytes, const void **d_row)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    const Plan *plan = reinterpret_cast<const Plan *>(plan_);
+    if (!plan || !P || !shard || !row_bytes)
+    {
+        set_error(-3, "krep_b200_regex_export_shard: null argument");
+        return -3;
+    }
+    DeviceGuard guard;
+    if (stream && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+    {
+        set_error(-2, "krep_b200_regex_export_shard: the caller's stream failed (%s)", cudaGetErrorString(cudaGetLastError()));
+        return -2;
+    }
+    t_rx_stats = RegexPackStats();
+    DevCtx *C = nullptr;
+    const void *row = nullptr;
+    int rc = regex_export(plan, P, shard, "krep_b200_regex_export_shard", &C, &row, row_bytes);
+    if (rc != 0) return rc;
+    if (d_row) *d_row = row;
+    if (!dst) return 0;
+    if (dst_cap < *row_bytes)
+    {
+        set_error(-5, "krep_b200_regex_export_shard: the row needs %llu bytes, dst has %llu", (unsigned long long)*row_bytes,
+                  (unsigned long long)dst_cap);
+        return -5;
+    }
+    CKH(cudaMemcpyAsync(dst, row, *row_bytes, cudaMemcpyDefault, C->scan_stream));
+    CKH(cudaStreamSynchronize(C->scan_stream));
+    return 0;
+}
+
+uint64_t krep_b200_regex_resolve(const search_params_t *P, const void *const *rows, uint32_t n_rows, match_result_t *result)
+{
+    clear_error();
+    if (!P) return 0;
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
+    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    int err = 0;
+    const uint64_t ret = regex_resolve_rows(P, rows, n_rows, result, &err);
+    return err ? 0 : ret;
+}
+
+void krep_b200_regex_export_stats(float *scan_ms, float *pack_ms, uint64_t *packed_bytes)
+{
+    if (scan_ms) *scan_ms = t_rx_stats.scan_ms;
+    if (pack_ms) *pack_ms = t_rx_stats.pack_ms;
+    if (packed_bytes) *packed_bytes = t_rx_stats.packed_bytes;
 }
 
 // ---- test hook: the line filter of a regex plan, run on the host ----

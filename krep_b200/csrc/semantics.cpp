@@ -7,6 +7,7 @@
 // does in find_line_start/find_line_end, krep.c:363-408).
 #define _GNU_SOURCE
 #include <algorithm>
+#include <cassert>
 #include <cstdlib>
 #include <cstring>
 #include <cstdio>
@@ -572,6 +573,19 @@ uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *re
 // flagged lines the cursor is in: [cur, E) with E the byte after the run's last newline, and REG_NOTEOL when E is not
 // the end of the text, so that '$' cannot match at a false end of string.  Every match, and every -w / -c / -m
 // decision, is glibc's own on the caller's regex_t.  r.keys are the flagged line starts (ascending, global offsets).
+//
+// Windowed (r.window_len set, resident shards): r.text holds only [origin, origin + window_len), and every run the keys
+// form lies inside it.  The replay never reads outside the window (WINDOW_ASSERT in debug builds) because:
+//   * REG_NOTEOL depends on the run ending before the TRUE end of the text (n), not before the end of the window;
+//   * the byte before a run is the '\n' that ends the previous line (or there is none), so at_line_start and -w's
+//     is_word_c(t[start - 1]) read the window for every start above its origin and know the answer at the origin; -w's
+//     t[end] lies inside too: a match never contains '\n', so it ends at or before the '\n' that ends its line;
+//   * the empty string at n is decided from r.last_byte when the window does not hold the text's last byte.
+#ifdef KREP_B200_DEBUG
+#define WINDOW_ASSERT(c) assert(c)
+#else
+#define WINDOW_ASSERT(c) ((void)0)
+#endif
 uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res)
 {
     if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0;
@@ -595,10 +609,23 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
     const int base_eflags = REG_STARTEND | REG_NEWLINE | (P->case_sensitive ? 0 : REG_ICASE);
     const size_t max_count = P->max_count;
     const size_t RUN_MAX = (size_t)1 << 30; // regoff_t is an int: a run is cut (at a line start) before it gets near 2^31
+    const size_t org = r.origin, wend = r.window_len == SIZE_MAX ? n : org + r.window_len; // t[x - org] is byte x
+    auto at = [&](size_t x) {
+        WINDOW_ASSERT(x >= org && x < wend);
+        return (unsigned char)t[x - org];
+    };
     auto key_pos = [&](size_t j) { return (size_t)((r.keys[j] >> LIT_TAG_BITS) - r.base); };
     auto after_line = [&](size_t s) {
-        const size_t e = line_end(t, n, s);
-        return e < n ? e + 1 : n;
+        if (s >= n) return n;
+        WINDOW_ASSERT(s >= org && s <= wend);
+        const void *nl = s < wend ? memchr(t + (s - org), '\n', wend - s) : nullptr;
+        WINDOW_ASSERT(nl || wend == n); // a window holds whole lines
+        return nl ? (size_t)((const char *)nl - t) + org + 1 : n;
+    };
+    auto first_of_line = [&](size_t s) { // line_start(): a window starts at a line start
+        WINDOW_ASSERT(s >= org && s <= wend);
+        const void *nl = s > org ? memrchr(t, '\n', s - org) : nullptr;
+        return nl ? (size_t)((const char *)nl - t) + org + 1 : org;
     };
     size_t ki = 0, run_end = 0, cur = 0, last_line = SIZE_MAX;
     uint64_t count = 0;
@@ -621,7 +648,7 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
                 // no flagged line left.  A text that ends with '\n' still has an empty string after it, where the
                 // reference's search from the cursor can end with an empty match (^ or $ at the end of the text) —
                 // unless that end belongs to another decider
-                if (t[n - 1] != '\n' || r.stop < n) break;
+                if (r.stop < n || (r.last_byte >= 0 ? r.last_byte : at(n - 1)) != '\n') break;
                 s = e = n;
             }
             const size_t run_start = s;
@@ -632,9 +659,10 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
         regmatch_t pmatch[1];
         pmatch[0].rm_so = 0;
         pmatch[0].rm_eo = (regoff_t)(run_end - cur);
-        const bool at_line_start = cur == 0 || t[cur - 1] == '\n';
+        const bool at_line_start = cur == org || at(cur - 1) == '\n'; // the byte before a window is a '\n' (or none)
         const int eflags = base_eflags | (at_line_start ? 0 : REG_NOTBOL) | (run_end < n ? REG_NOTEOL : 0);
-        const int rc = regexec(regex, t + cur, 1, pmatch, eflags);
+        WINDOW_ASSERT(cur >= org && run_end <= wend);
+        const int rc = regexec(regex, t + (cur - org), 1, pmatch, eflags);
         if (rc != 0)
         {
             if (rc == REG_NOMATCH)
@@ -667,14 +695,14 @@ uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t 
             cur = run_end;
             continue;
         }
-        if (P->whole_word && ((start > 0 && is_word_c((unsigned char)t[start - 1])) || (end < n && is_word_c((unsigned char)t[end]))))
+        if (P->whole_word && ((start > org && is_word_c(at(start - 1))) || (end < n && is_word_c(at(end)))))
         {
             cur = std::min(cur + so + 1, n); // krep.c:1487-1501
             continue;
         }
         if (P->count_lines_mode)
         {
-            const size_t ls = line_start(t, n, start);
+            const size_t ls = first_of_line(start);
             if (ls != last_line)
             {
                 count++;
@@ -752,6 +780,108 @@ uint64_t replay_regex_matches(const search_params_t *P, const Replay &r, match_r
         Replay g{lines.data(), lines.size(), t, n, 0};
         g.stop = end < n ? end : SIZE_MAX;
         count += replay_regex(&sub, g, res);
+    }
+    return count;
+}
+
+// Windowed replays (resident shards, DESIGN §12.4).  Running replay_regex window by window gives what one call over the
+// whole text gives: a window starts at a line start, and a run cut there behaves as the RUN_MAX cut does — every call
+// but the one whose window ends at n has stop set, so an empty match at its clipped end ('^' after its last '\n') is left
+// to the next window, where the whole-text replay also finds it (from that line's start, the next run's start).  The
+// cursor, the -m budget and (for -c) the last counted line carry over: a line lies in one window only.
+uint64_t replay_regex_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w, size_t nw,
+                              size_t n, int last_byte, bool at_end, match_result_t *res)
+{
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0;
+    const size_t max_count = P->max_count;
+    uint64_t count = 0;
+    size_t j = 0, covered = 0; // covered: end of the last window replayed
+    for (size_t i = 0; i < nw && j < nkeys && count < max_count; i++)
+    {
+        const size_t wb = w[i].origin, we = wb + w[i].len;
+        while (j < nkeys && (size_t)(keys[j] >> LIT_TAG_BITS) < wb) j++; // a key outside every window: not a line glibc sees
+        const size_t j0 = j;
+        while (j < nkeys && (size_t)(keys[j] >> LIT_TAG_BITS) < we) j++;
+        if (j == j0) continue;
+        search_params_t sub = *P;
+        sub.max_count = max_count - count;
+        Replay g{keys + j0, j - j0, w[i].bytes, n, 0};
+        g.origin = wb;
+        g.window_len = w[i].len;
+        g.stop = we < n ? we : SIZE_MAX;
+        g.last_byte = last_byte;
+        count += replay_regex(&sub, g, res);
+        covered = we;
+    }
+    // The empty string at n: the whole-text replay tries it once its keys run out before n, if the text ends in '\n'
+    // and the budget allows.  A last window that ends at n has decided it already; otherwise one call with no keys and
+    // an empty window at n does, from the last byte of the text.
+    if (at_end && count < max_count && covered < n && n > 0)
+    {
+        search_params_t sub = *P;
+        sub.max_count = max_count - count;
+        Replay g{nullptr, 0, "", n, 0};
+        g.origin = n;
+        g.window_len = 0;
+        g.last_byte = last_byte;
+        count += replay_regex(&sub, g, res);
+    }
+    return count;
+}
+
+// replay_regex_matches over windows: the same walk; a stretch of uncertain lines goes through replay_regex_windows, whose
+// windows (runs of uncertain lines) end where the stretch ends, so the stop rule is the one the whole-text walk applies.
+uint64_t replay_regex_matches_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w,
+                                      size_t nw, size_t n, int last_byte, match_result_t *res)
+{
+    const uint64_t max_count = P->max_count;
+    std::vector<uint64_t> lines;
+    uint64_t count = 0;
+    size_t i = 0, wi = 0;
+    while (i < nkeys && count < max_count)
+    {
+        const uint64_t k = keys[i];
+        const size_t pos = (size_t)(k >> REGEX_MATCH_SHIFT);
+        if (k & 1)
+        {
+            const size_t len = (size_t)((k >> LIT_TAG_BITS) & ((1u << (REGEX_MATCH_SHIFT - LIT_TAG_BITS)) - 1));
+            count++;
+            if (res) result_push(res, pos, pos + len);
+            i++;
+            continue;
+        }
+        lines.clear();
+        size_t end = 0;
+        while (wi < nw && w[wi].origin + w[wi].len <= pos) wi++;
+        size_t wj = wi;
+        while (i < nkeys)
+        {
+            const uint64_t u = keys[i];
+            const size_t s = (size_t)(u >> REGEX_MATCH_SHIFT);
+            if (u & 1)
+            {
+                if (s < end)
+                {
+                    i++;
+                    continue;
+                }
+                break;
+            }
+            lines.push_back((uint64_t)s << LIT_TAG_BITS);
+            // the end of the line at s, from the window that holds it
+            while (wj < nw && w[wj].origin + w[wj].len <= s) wj++;
+            end = n;
+            if (wj < nw && w[wj].origin <= s)
+            {
+                const size_t off = s - w[wj].origin;
+                const void *nl = memchr(w[wj].bytes + off, '\n', w[wj].len - off);
+                if (nl) end = w[wj].origin + (size_t)((const char *)nl - w[wj].bytes) + 1;
+            }
+            i++;
+        }
+        search_params_t sub = *P;
+        sub.max_count = (size_t)(max_count - count);
+        count += replay_regex_windows(&sub, lines.data(), lines.size(), w + wi, nw - wi, n, last_byte, false, res);
     }
     return count;
 }

@@ -114,6 +114,12 @@ def load():
     L.krep_b200_regex_scan_shard_raw.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.POINTER(C.c_uint64), C.c_uint64,
                                                  C.POINTER(C.c_uint64)]
     L.krep_b200_regex_scan_shard_raw.restype = C.c_int64
+    L.krep_b200_regex_export_shard.argtypes = [C.c_void_p, C.POINTER(SearchParams), C.POINTER(Shard), C.c_void_p, C.c_void_p,
+                                               C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_void_p)]
+    L.krep_b200_regex_export_shard.restype = C.c_int
+    L.krep_b200_regex_resolve.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(MatchResult)]
+    L.krep_b200_regex_resolve.restype = C.c_uint64
+    L.krep_b200_regex_export_stats.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64)]
     L.krep_b200_last_kernel_ms.restype = C.c_float
     L.krep_b200_launch_count.restype = C.c_uint64
     for n in ("krep_b200_ac_key_end", "krep_b200_ac_key_start"):
@@ -226,3 +232,37 @@ def search_batch(func, params, texts, with_result=True):
             L.krep_b200_ac_trie_free(params.struct.ac_trie)
             params.struct.ac_trie = None
         L.krep_b200_set_only_matching(False)
+
+
+def _positions(res):
+    r = res.contents
+    return [(r.positions[i].start_offset, r.positions[i].end_offset) for i in range(r.count)]
+
+
+def search_shards(plan, params, shards, with_result=True):
+    """krep_b200_search_shards on a list of Shard structs (text order). -> (count, [(start, end), ...])"""
+    L = load()
+    arr = (Shard * max(len(shards), 1))(*shards)
+    res = L.krep_b200_match_result_init(16) if with_result else None
+    try:
+        cnt = L.krep_b200_search_shards(plan, params.ref(), arr, len(shards), res)
+        check(L)
+        return int(cnt), (_positions(res) if res else [])
+    finally:
+        if res:
+            L.krep_b200_match_result_free(res)
+
+
+def regex_resolve(params, rows, with_result=True):
+    """krep_b200_regex_resolve over host rows (bytes objects, text order). -> (count, [(start, end), ...])"""
+    L = load()
+    bufs = [C.create_string_buffer(bytes(r), max(len(r), 1)) for r in rows]
+    arr = (C.c_void_p * max(len(rows), 1))(*[C.cast(b, C.c_void_p) for b in bufs])
+    res = L.krep_b200_match_result_init(16) if with_result else None
+    try:
+        cnt = L.krep_b200_regex_resolve(params.ref(), arr, len(rows), res)
+        check(L)
+        return int(cnt), (_positions(res) if res else [])
+    finally:
+        if res:
+            L.krep_b200_match_result_free(res)
