@@ -164,11 +164,27 @@ uint64_t krep_b200_regex_search(const search_params_t *, const char *, size_t, m
 
 /* Many texts, one launch — what search_directory_recursive (krep.c:3310) calling search_file once per small file
  * becomes when the per-call copy and launch latency matters.  `entry` is one of the literal and pattern-set functions
- * above (not krep_b200_regex_search, which is refused with an error); text i gets
+ * above (not krep_b200_regex_search, which is refused with an error: -E batches go through
+ * krep_b200_regex_search_batch); text i gets
  * exactly the count (counts[i]) and positions (results[i], may be NULL, or results == NULL) that
  * entry(params, texts[i], lens[i], results[i]) would have produced.  Returns 0, or a negative error. */
 int krep_b200_search_batch(search_func_t entry, const search_params_t *params, const char *const *texts,
                            const size_t *lens, size_t n_texts, uint64_t *counts, match_result_t *const *results);
+
+/* -E over many texts in one pack, one copy and one scan.  For every i, counts[i] and results[i] (results or results[i]
+ * may be NULL) are exactly what krep_b200_regex_search(params, texts[i], lens[i], results[i]) returns: the count, the
+ * positions and their order, on each of its three paths (fused -c, offsets on the GPU, line filter + regexec), chosen
+ * once per call from params and switched by the same KREP_B200_NO_FUSED_COUNT / KREP_B200_NO_DEVICE_MATCHES.  Per text:
+ * its own -m budget, -w, -i, -c, -co, and the early returns (max_count == 0, no compiled_regex, the empty text), which
+ * are answered on the host without a launch.  The texts are packed at 16-byte aligned offsets with '\n' gaps, so no line
+ * crosses from one text into the next; every text still costs at least one regexec call on its last line on the -c and
+ * offsets paths.  A pattern krep_b200_regex_search refuses fails the call with -3 and every count 0.  Returns 0, or a
+ * negative error. */
+int krep_b200_regex_search_batch(const search_params_t *params, const char *const *texts, const size_t *lens,
+                                 size_t n_texts, uint64_t *counts, match_result_t *const *results);
+/* Host-clock times of the calling thread's most recent krep_b200_regex_search_batch: packing the texts (with the text
+ * table) and the per-text replays.  The scan itself is krep_b200_last_kernel_ms. */
+void krep_b200_regex_batch_stats(double *pack_ms, double *resolve_ms);
 
 /* krep.c:1771 — same decision order, same globals.  For use_regex it returns
  * krep_b200_regex_search when the pattern's line automaton compiles, and
@@ -424,6 +440,14 @@ int64_t krep_b200_regex_matches_host(const search_params_t *params, const char *
  * No search entry point calls it. */
 int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
                                        uint64_t *keys, uint64_t cap, uint64_t *device_lines);
+/* Test hook: one batch scan of krep_b200_regex_search_batch in `mode` (0, 1, 2 as above) over the texts with lens[i] > 0.
+ * offsets[i] (may be NULL): text i's packed offset (UINT64_MAX for a text not packed); keys[0 .. min(result, cap)):
+ * the sorted keys in packed coordinates; text_lines[i] (may be NULL): in mode 1 the lines of text i decided MATCHED on
+ * the device (else 0).  Returns the exact number of keys, or a negative error (refused pattern, or a mode the pattern
+ * does not admit).  No search entry point calls it. */
+int64_t krep_b200_regex_search_batch_raw(const search_params_t *params, const char *const *texts, const size_t *lens,
+                                         size_t n_texts, int mode, uint64_t *offsets, uint64_t *keys, uint64_t cap,
+                                         uint64_t *text_lines);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

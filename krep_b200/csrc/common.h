@@ -165,6 +165,21 @@ struct RegexLaunch
     unsigned long long *line_count; // count mode (-c): lines decided MATCHED on the device; nullptr = filter mode
     // match mode (offsets on the device) when set: the match table follows the class map in `trans`
     uint32_t matches, nmtrans, match_bol, match_mid;
+    // batch mode when text_end is set (krep_b200_regex_search_batch, DESIGN §12.5): the text holds many texts packed at
+    // 16-byte aligned global offsets, each followed by '\n' bytes up to the next text; a line belongs to the text it
+    // starts in, and its uncertain-line rule and -c counter are that text's own
+    const uint64_t *text_start, *text_end; // global [start, end) of packed text i, ascending
+    const uint32_t *seg_text;              // per global 256-byte segment g: the first text i with text_end[i] > g * 256
+    unsigned long long *text_lines;        // count mode: lines of text i decided MATCHED (replaces line_count)
+    uint32_t n_texts;
+};
+static_assert(REGEX_SEG == 256, "RegexLaunch::seg_text has one entry per 256 bytes");
+// The device copies of a batch's text table (RegexLaunch batch fields), handed to launch_scan.
+struct RegexBatchDev
+{
+    const uint64_t *text_start, *text_end;
+    const uint32_t *seg_text;
+    uint32_t n_texts;
 };
 
 struct AcDevTables;  // scan_multi.cu: one device's copy of a pattern set's tables
@@ -237,8 +252,9 @@ static constexpr uint64_t LB_OUTSIDE_SHARD = ~0ull - 2; // the line continues in
 // Launch one shard scan on `stream` of the device context; appends to that device's key list (no counter reset).
 // regex_lines (regex plans only): run k_regex_lines in count mode, adding the lines it decides MATCHED there.
 // regex_matches (offsets_exact regex plans, with want_positions): run it in match mode (match and uncertain-line keys).
+// regex_batch: the shard is (a chunk of) a packed batch of texts; regex_lines then has one counter per text.
 int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0,
-                unsigned long long *regex_lines = nullptr, bool regex_matches = false);
+                unsigned long long *regex_lines = nullptr, bool regex_matches = false, const RegexBatchDev *regex_batch = nullptr);
 // literal kernels (scan_literal.cu)
 void launch_literal(const Plan *plan, const LitDevParams &p, int sm_count, cudaStream_t s);
 // multi kernels (scan_multi.cu)

@@ -266,6 +266,7 @@ static void ctx_destroy(DevCtx &E)
     cudaFree(E.d_bounds);
     cudaFreeHost(E.h_bounds);
     cudaFreeHost(E.h_batch);
+    cudaFree(E.d_rx_batch);
     cudaFree(E.d_counter);
     cudaFree(E.d_ring);
     cudaFree(E.d_line_recs);
@@ -583,7 +584,7 @@ Plan *plan_build(const search_params_t *P, int algo, bool only_matching)
 // shard scan
 // ---------------------------------------------------------------------------------------------
 int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot,
-                unsigned long long *regex_lines, bool regex_matches)
+                unsigned long long *regex_lines, bool regex_matches, const RegexBatchDev *regex_batch)
 {
     if (((uintptr_t)sh->d_text & 15) != 0)
     {
@@ -622,11 +623,16 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.out = E.d_list[slot];
         a.cap = want_positions ? E.key_cap : 0;
         a.counter = slot_counter(E, slot);
-        a.line_count = regex_lines;
+        a.line_count = regex_batch ? nullptr : regex_lines;
         a.matches = regex_matches ? 1u : 0u;
         a.nmtrans = (uint32_t)plan->rx->match.size();
         a.match_bol = plan->rx->match_bol;
         a.match_mid = plan->rx->match_mid;
+        a.text_start = regex_batch ? regex_batch->text_start : nullptr;
+        a.text_end = regex_batch ? regex_batch->text_end : nullptr;
+        a.seg_text = regex_batch ? regex_batch->seg_text : nullptr;
+        a.text_lines = regex_batch ? regex_lines : nullptr;
+        a.n_texts = regex_batch ? regex_batch->n_texts : 0u;
         launch_regex(a, E.sm_count, stream);
         return 0;
     }

@@ -80,6 +80,8 @@ struct DevCtx
     uint64_t h_keys_cap = 0;
     uint8_t *h_batch = nullptr; // pinned: texts of one krep_b200_search_batch call, packed
     uint64_t h_batch_cap = 0;
+    uint8_t *d_rx_batch = nullptr; // the text table of a krep_b200_regex_search_batch call (RegexBatchDev)
+    size_t rx_batch_cap = 0;
     RegexPackBufs *rx_pack = nullptr; // -E rows of resident shards (scan_regex_pack.cu)
 };
 

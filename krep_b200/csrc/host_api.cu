@@ -9,6 +9,7 @@
 // kernels append to one device occurrence list, which is sorted on the device, read back, and replayed
 // under the emulated kernel's policy (semantics.cpp).  There is no CPU scan anywhere on this path.
 #include <algorithm>
+#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -298,6 +299,34 @@ void prewarm_host_path(DevCtx &E)
 // reads cost nothing) and taking its -w context bytes straight from the host text.  All chunk scans of the device
 // append to one occurrence list; k_finish / the radix sort order it.  If the list overflows, it is grown and the
 // range is staged again.
+// The text table of a packed -E batch (DESIGN §12.5), global offsets: text i is [start[i], end[i]), and seg[g] is the
+// first text i with end[i] > g * REGEX_SEG (n_texts when there is none).
+struct RegexBatch
+{
+    std::vector<uint64_t> start, end;
+    std::vector<uint32_t> seg;
+};
+
+// Copies the table to the device (on its scan stream, behind the scans before it).
+static int upload_regex_batch(DevCtx &E, const RegexBatch &B, RegexBatchDev *out)
+{
+    const size_t nt = B.end.size(), bytes = nt * 16 + B.seg.size() * 4;
+    if (bytes > E.rx_batch_cap)
+    {
+        cudaFree(E.d_rx_batch);
+        E.d_rx_batch = nullptr;
+        E.rx_batch_cap = 0;
+        CKH(cudaMalloc(&E.d_rx_batch, bytes + bytes / 4));
+        E.rx_batch_cap = bytes + bytes / 4;
+    }
+    uint64_t *d = (uint64_t *)E.d_rx_batch;
+    CKH(cudaMemcpyAsync(d, B.start.data(), nt * 8, cudaMemcpyHostToDevice, E.scan_stream));
+    CKH(cudaMemcpyAsync(d + nt, B.end.data(), nt * 8, cudaMemcpyHostToDevice, E.scan_stream));
+    CKH(cudaMemcpyAsync(d + 2 * nt, B.seg.data(), B.seg.size() * 4, cudaMemcpyHostToDevice, E.scan_stream));
+    *out = RegexBatchDev{d, d + nt, (const uint32_t *)(d + 2 * nt), (uint32_t)nt};
+    return 0;
+}
+
 struct RangeJob
 {
     DevCtx *C = nullptr;
@@ -311,6 +340,8 @@ struct RangeJob
     bool regex_count = false; // fused -E -c: every chunk adds its device-decided matching lines and leaves its uncertain keys
     uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
     bool regex_matches = false; // -E offsets on the device: match keys and uncertain-line keys (REGEX_MATCH_SHIFT layout)
+    const RegexBatch *batch = nullptr; // -E batch: the text is packed texts; regex_count then counts per text
+    std::vector<uint64_t> text_lines;  // batch, fused -c: lines of each text decided MATCHED in this range
     // results
     int rc = 0;
     ScanOut so;
@@ -336,15 +367,19 @@ static int stream_range(RangeJob &J)
     if (!J.pinned && ensure_stage(E, std::min(chunk, span) + halo + 64, nslots) != 0) return -2;
     if (J.want_positions && ensure_keys(E, 1) != 0) return -2;
     if (J.count_lines && ensure_line_out(E, nchunks) != 0) return -2;
-    if (J.regex_count && ensure_line_out(E, 1) != 0) return -2; // the range's line counter: d_line_out[0]
+    // the range's line counter: d_line_out[0] (a batch: one per text, d_line_out[0 .. n_texts))
+    const size_t n_lines = J.batch ? J.batch->end.size() : 1;
+    if (J.regex_count && ensure_line_out(E, (n_lines + 1) / 2) != 0) return -2;
     unsigned long long *d_regex_lines = J.regex_count ? (unsigned long long *)E.d_line_out : nullptr;
+    RegexBatchDev batch_dev{};
+    if (J.batch && upload_regex_batch(E, *J.batch, &batch_dev) != 0) return -2;
     reset_kernel_ms();
     const int slot = 0;
     for (int attempt = 0; attempt < 3; attempt++)
     {
         CKH(cudaStreamWaitEvent(E.scan_stream, E.ev_done[slot], 0));
         if (reset_counter(E, slot, E.scan_stream) != 0) return -2;
-        if (d_regex_lines) CKH(cudaMemsetAsync(d_regex_lines, 0, sizeof(unsigned long long), E.scan_stream)); // also on a re-stage
+        if (d_regex_lines) CKH(cudaMemsetAsync(d_regex_lines, 0, n_lines * sizeof(unsigned long long), E.scan_stream)); // also on a re-stage
         for (size_t c = 0; c < nchunks; c++)
         {
             const size_t off = J.begin + c * chunk, len = std::min(chunk, J.end - off);
@@ -377,14 +412,15 @@ static int stream_range(RangeJob &J)
             CKH(cudaEventRecord(a, E.scan_stream));
             int rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
                                    : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines,
-                                                 J.regex_matches);
+                                                 J.regex_matches, J.batch ? &batch_dev : nullptr);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
             CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
         }
         CKH(cudaGetLastError());
         if (!J.count_lines && finish_scan(E, slot, J.want_positions, E.scan_stream) != 0) return -2;
-        if (d_regex_lines) CKH(cudaMemcpyAsync(E.h_line_out, d_regex_lines, sizeof(uint64_t), cudaMemcpyDeviceToHost, E.scan_stream));
+        if (d_regex_lines)
+            CKH(cudaMemcpyAsync(E.h_line_out, d_regex_lines, n_lines * sizeof(uint64_t), cudaMemcpyDeviceToHost, E.scan_stream));
         CKH(cudaStreamSynchronize(E.scan_stream));
         if (!J.count_lines) CKH(cudaEventSynchronize(E.ev_done[slot])); // k_finish runs on the finish stream
         for (auto &s : E.stage) s.in_flight = false;
@@ -400,7 +436,8 @@ static int stream_range(RangeJob &J)
             J.so = ScanOut();
             return 0;
         }
-        if (J.regex_count) J.regex_lines = E.h_line_out[0];
+        if (J.regex_count && J.batch) J.text_lines.assign(E.h_line_out, E.h_line_out + n_lines);
+        else if (J.regex_count) J.regex_lines = E.h_line_out[0];
         const uint64_t cnt = E.h_pack[slot][0];
         J.so = ScanOut();
         J.so.count = cnt;
@@ -465,13 +502,15 @@ struct HostScan
     uint64_t nkeys = 0;
     std::vector<uint64_t> merged; // backing store when several devices contributed
     uint64_t regex_lines = 0;     // fused -E -c: lines decided MATCHED on the devices (the keys are the uncertain lines)
+    std::vector<uint64_t> text_lines; // the same per text of a batch
 };
 
 // count_lines: the fused -c of the plan — a line record per chunk for literals; for regex plans a device line count per
 // range next to the keys of the uncertain lines (want_positions must then be set).  regex_matches: -E offsets on the
-// device (offsets_exact regex plans, want_positions set): the keys are match keys and uncertain-line keys.
+// device (offsets_exact regex plans, want_positions set): the keys are match keys and uncertain-line keys.  batch: the
+// text is a packed -E batch with this text table (DESIGN §12.5).
 static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want_positions, HostScan *hs, bool count_lines = false,
-                          bool regex_matches = false)
+                          bool regex_matches = false, const RegexBatch *batch = nullptr)
 {
     const bool pinned = is_pinned(text);
     const size_t chunk = pinned ? env_mb("KREP_B200_CHUNK_MB", 256) : env_mb("KREP_B200_STAGE_MB", 32);
@@ -505,6 +544,7 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.count_lines = count_lines && !plan->is_regex;
         J.regex_count = count_lines && plan->is_regex;
         J.regex_matches = regex_matches;
+        J.batch = batch;
     }
     trace("search: %zu bytes (%s host memory), %zu device(s), %zu range(s), chunk %zu MiB", n, pinned ? "pinned" : "pageable", D, R,
           chunk >> 20);
@@ -570,6 +610,14 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
     hs->keys = nullptr;
     hs->nkeys = 0;
     hs->regex_lines = 0;
+    hs->text_lines.clear();
+    if (batch && count_lines)
+    {
+        // every line is decided by one range: the per-text counts add up
+        hs->text_lines.assign(batch->end.size(), 0);
+        for (auto &J : jobs)
+            for (size_t i = 0; i < J.text_lines.size(); i++) hs->text_lines[i] += J.text_lines[i];
+    }
     if (count_lines && !plan->is_regex)
     {
         // chunk records of all ranges, in text order -> matching lines (a line cut by a chunk / range / device edge is
@@ -971,6 +1019,41 @@ static uint64_t search_shards_regex(const Plan *plan, const search_params_t *P, 
     return err ? 0 : ret;
 }
 
+// Packs texts[f] for f in `live` (ascending) into the device's pinned batch buffer with the staging threads: text f at the
+// 16-byte aligned (*off)[f], followed by at least `gap` bytes of `fill` up to the next text's offset (or *total).
+static int pack_texts(DevCtx &E, const char *const *texts, const size_t *lens, const std::vector<size_t> &live, size_t gap,
+                      uint8_t fill, std::vector<uint64_t> *off, uint64_t *total)
+{
+    uint64_t t = 0;
+    for (size_t f : live)
+    {
+        (*off)[f] = t;
+        t = (t + lens[f] + gap + 15) & ~15ull;
+    }
+    *total = t;
+    if (t > E.h_batch_cap)
+    {
+        cudaFreeHost(E.h_batch);
+        E.h_batch = nullptr;
+        E.h_batch_cap = 0;
+        CKH(cudaMallocHost(&E.h_batch, t + t / 4 + 4096));
+        E.h_batch_cap = t + t / 4 + 4096;
+    }
+    // only the gaps are filled
+    const long nl = (long)live.size();
+    uint8_t *const hb = E.h_batch;
+    const uint64_t *o = off->data();
+#pragma omp parallel for num_threads(copy_threads()) schedule(dynamic, 16)
+    for (long i = 0; i < nl; i++)
+    {
+        const size_t f = live[(size_t)i];
+        const uint64_t end = o[f] + lens[f], next = i + 1 < nl ? o[live[(size_t)i + 1]] : t;
+        memcpy(hb + o[f], texts[f], lens[f]);
+        memset(hb + end, fill, next - end);
+    }
+    return 0;
+}
+
 // Many texts, one launch (SURVEY §8 f4: small files lose to launch and copy latency one by one).  The texts are packed
 // into one pinned buffer at 16-byte aligned offsets, separated by zero gaps longer than the longest pattern, copied and
 // scanned as ONE shard; the sorted occurrence list is then cut per text — an occurrence belongs to a text only if it
@@ -1006,39 +1089,13 @@ static int run_batch(int entry_algo, const search_params_t *P, const char *const
     Plan *plan = plan_for(P, algo, only_matching);
     if (!plan) return -2;
     const size_t gap = (size_t)(plan->is_ac ? plan->max_len : plan->m) + 16;
+    std::vector<size_t> live;
+    for (size_t f = 0; f < nt; f++)
+        if (algo_of[f] >= 0) live.push_back(f);
     std::vector<uint64_t> off(nt, 0);
     uint64_t total = 0;
-    for (size_t f = 0; f < nt; f++)
-        if (algo_of[f] >= 0)
-        {
-            off[f] = total;
-            total = (total + lens[f] + gap + 15) & ~15ull;
-        }
     DevCtx &E = *Cp;
-    if (total > E.h_batch_cap)
-    {
-        cudaFreeHost(E.h_batch);
-        E.h_batch = nullptr;
-        E.h_batch_cap = 0;
-        CKH(cudaMallocHost(&E.h_batch, total + total / 4 + 4096));
-        E.h_batch_cap = total + total / 4 + 4096;
-    }
-    {
-        // pack with the staging threads; only the gaps are zeroed
-        std::vector<size_t> live;
-        for (size_t f = 0; f < nt; f++)
-            if (algo_of[f] >= 0) live.push_back(f);
-        const long nl = (long)live.size();
-        uint8_t *const hb = E.h_batch;
-#pragma omp parallel for num_threads(copy_threads()) schedule(dynamic, 16)
-        for (long i = 0; i < nl; i++)
-        {
-            const size_t f = live[(size_t)i];
-            const uint64_t end = off[f] + lens[f], next = i + 1 < nl ? off[live[(size_t)i + 1]] : total;
-            memcpy(hb + off[f], texts[f], lens[f]);
-            memset(hb + end, 0, next - end);
-        }
-    }
+    if (pack_texts(E, texts, lens, live, gap, 0, &off, &total) != 0) return -2;
     HostScan hs;
     if (stage_and_scan(plan, (const char *)E.h_batch, total, 1, &hs) != 0) return -2;
     const uint64_t *keys = hs.keys;
@@ -1076,6 +1133,124 @@ static int run_batch(int entry_algo, const search_params_t *P, const char *const
         match_result_t *res = results ? results[f] : nullptr;
         counts[f] = plan->is_ac ? replay_ac(P, r, res) : replay_literal(algo, P, only_matching, plan->m, r, res);
     }
+    return 0;
+}
+
+// ---- -E over many texts (DESIGN §12.5) ----
+struct RegexBatchTimes
+{
+    double pack_ms = 0, resolve_ms = 0; // host clock: packing (with the text table), and the per-text replays
+};
+static thread_local RegexBatchTimes t_rx_batch; // of the most recent krep_b200_regex_search_batch call
+
+static double ms_since(std::chrono::steady_clock::time_point t0)
+{
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
+// One k_regex_lines scan in `mode` (0 filter, 1 fused -c, 2 offsets) of the texts f in `live` (ascending, lens[f] > 0):
+// packed with '\n' gaps (at least one '\n' after each text, up to the next 16-byte boundary), so that no line and no
+// automaton walk crosses from one text into the next, and scanned by stage_and_scan as one text in the kernel's batch
+// mode.  *off (indexed by f): packed offsets; *hs: the sorted keys in packed coordinates and, in mode 1, the device line
+// count of each live text (indexed like `live`).
+static int regex_batch_scan(const Plan *plan, const char *const *texts, const size_t *lens, const std::vector<size_t> &live,
+                            int mode, const char *who, std::vector<uint64_t> *off, HostScan *hs)
+{
+    if (live.size() >= UINT32_MAX)
+    {
+        set_error(-3, "%s: too many texts in one call", who);
+        return -3;
+    }
+    DevCtx *Cp = ctx_primary();
+    if (!Cp) return -1;
+    const auto t0 = std::chrono::steady_clock::now();
+    uint64_t total = 0;
+    if (pack_texts(*Cp, texts, lens, live, 1, '\n', off, &total) != 0) return -2;
+    // the text table; seg[g]: the first text that ends after g * REGEX_SEG
+    RegexBatch B;
+    const size_t nl = live.size();
+    B.start.resize(nl);
+    B.end.resize(nl);
+    for (size_t i = 0; i < nl; i++)
+    {
+        B.start[i] = (*off)[live[i]];
+        B.end[i] = B.start[i] + lens[live[i]];
+    }
+    B.seg.resize((total + REGEX_SEG - 1) / REGEX_SEG);
+    for (size_t g = 0, i = 0; g < B.seg.size(); g++)
+    {
+        while (i < nl && B.end[i] <= (uint64_t)g * REGEX_SEG) i++;
+        B.seg[g] = (uint32_t)i;
+    }
+    t_rx_batch.pack_ms += ms_since(t0);
+    trace("regex batch: %zu texts packed into %llu bytes", nl, (unsigned long long)total);
+    return stage_and_scan(plan, (const char *)Cp->h_batch, total, 1, hs, mode == 1, mode == 2, &B);
+}
+
+// krep_b200_regex_search_batch: text i gets krep_b200_regex_search(P, texts[i], lens[i], results[i])'s answer.  The
+// early returns are answered on the host; the other texts take one batch scan in the mode regex_call_mode picks for P,
+// and each text is then replayed on its own bytes with its own keys (Replay::base = its packed offset): its own -m
+// budget, its own last line and end-of-text quirks (the kernel leaves each text's last line uncertain).
+static int run_regex_batch(const search_params_t *P, const char *const *texts, const size_t *lens, size_t nt, uint64_t *counts,
+                           match_result_t *const *results)
+{
+    warm_join();
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    t_rx_batch = RegexBatchTimes();
+    if (!P || (nt && (!texts || !lens || !counts)))
+    {
+        set_error(-3, "krep_b200_regex_search_batch: null argument");
+        return -3;
+    }
+    for (size_t f = 0; f < nt; f++) counts[f] = 0;
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
+    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    std::vector<size_t> live;
+    for (size_t f = 0; f < nt; f++)
+        if (lens[f] > 0 && texts[f]) live.push_back(f);
+    DeviceGuard guard;
+    if (!live.empty())
+    {
+        if (visible_devices() == 0)
+        {
+            set_error(-1, "no CUDA device available; this engine has no CPU fallback");
+            return -1;
+        }
+        std::string why;
+        Plan *plan = cached_regex_plan(P, &why);
+        if (!plan)
+        {
+            set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
+            return -3;
+        }
+        const int mode = regex_call_mode(P, plan);
+        std::vector<uint64_t> off(nt, 0);
+        HostScan hs;
+        const int rc = regex_batch_scan(plan, texts, lens, live, mode, "krep_b200_regex_search_batch", &off, &hs);
+        if (rc != 0) return rc;
+        const auto t0 = std::chrono::steady_clock::now();
+        // keys ascend in packed coordinates: one pass cuts them per text (nothing outside a text is kept)
+        const int shift = mode == 2 ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+        size_t j = 0;
+        for (size_t i = 0; i < live.size(); i++)
+        {
+            const size_t f = live[i];
+            const uint64_t lo = off[f], hi = off[f] + lens[f];
+            while (j < hs.nkeys && (hs.keys[j] >> shift) < lo) j++;
+            size_t k = j;
+            while (k < hs.nkeys && (hs.keys[k] >> shift) < hi) k++;
+            const Replay r{hs.keys + j, k - j, texts[f], lens[f], lo};
+            match_result_t *res = results ? results[f] : nullptr;
+            counts[f] = mode == 2 ? replay_regex_matches(P, r, res) : mode == 1 ? regex_count_total(P, hs.text_lines[i], r) : replay_regex(P, r, res);
+            j = k;
+        }
+        t_rx_batch.resolve_ms = ms_since(t0);
+        trace("regex batch: mode %d, %zu texts, %llu keys (resolved in %.3f ms)", mode, live.size(), (unsigned long long)hs.nkeys,
+              t_rx_batch.resolve_ms);
+    }
+    for (size_t f = 0; f < nt; f++)
+        if (lens[f] == 0) counts[f] = replay_regex(P, Replay{nullptr, 0, texts[f], 0, 0}, results ? results[f] : nullptr); // krep.c:1403
     return 0;
 }
 
@@ -1146,7 +1321,7 @@ int krep_b200_search_batch(search_func_t entry, const search_params_t *params, c
     else if (entry == krep_b200_neon_search) algo = KREP_B200_ALGO_NEON;
     if (entry == krep_b200_regex_search)
     {
-        set_error(-3, "krep_b200_search_batch: regex searches are not batched; call krep_b200_regex_search per text");
+        set_error(-3, "krep_b200_search_batch: regex searches are batched by krep_b200_regex_search_batch");
         return -3;
     }
     if (algo < 0)
@@ -1155,6 +1330,59 @@ int krep_b200_search_batch(search_func_t entry, const search_params_t *params, c
         return -3;
     }
     return run_batch(algo, params, texts, lens, n_texts, counts, results);
+}
+
+int krep_b200_regex_search_batch(const search_params_t *params, const char *const *texts, const size_t *lens, size_t n_texts,
+                                 uint64_t *counts, match_result_t *const *results)
+{
+    return run_regex_batch(params, texts, lens, n_texts, counts, results);
+}
+
+void krep_b200_regex_batch_stats(double *pack_ms, double *resolve_ms)
+{
+    if (pack_ms) *pack_ms = t_rx_batch.pack_ms;
+    if (resolve_ms) *resolve_ms = t_rx_batch.resolve_ms;
+}
+
+// One batch scan in the given mode, its keys sorted and read back (DESIGN §12.5).
+int64_t krep_b200_regex_search_batch_raw(const search_params_t *P, const char *const *texts, const size_t *lens, size_t n_texts,
+                                         int mode, uint64_t *offsets, uint64_t *keys, uint64_t cap, uint64_t *text_lines)
+{
+    warm_join();
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    if (!P || (n_texts && (!texts || !lens)) || (cap && !keys))
+    {
+        set_error(-3, "krep_b200_regex_search_batch_raw: null argument");
+        return -3;
+    }
+    std::string why;
+    Plan *plan = cached_regex_plan(P, &why);
+    if (!plan || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    {
+        set_error(-3, "krep_b200_regex_search_batch_raw: mode %d is not available for this pattern", mode);
+        return -3;
+    }
+    std::vector<size_t> live;
+    for (size_t f = 0; f < n_texts; f++)
+    {
+        if (lens[f] > 0 && texts[f]) live.push_back(f);
+        if (offsets) offsets[f] = UINT64_MAX;
+        if (text_lines) text_lines[f] = 0;
+    }
+    if (live.empty()) return 0;
+    DeviceGuard guard;
+    std::vector<uint64_t> off(n_texts, 0);
+    HostScan hs;
+    const int rc = regex_batch_scan(plan, texts, lens, live, mode, "krep_b200_regex_search_batch_raw", &off, &hs);
+    if (rc != 0) return rc;
+    for (size_t i = 0; i < live.size(); i++)
+    {
+        if (offsets) offsets[live[i]] = off[live[i]];
+        if (text_lines && mode == 1) text_lines[live[i]] = hs.text_lines[i];
+    }
+    if (hs.nkeys && cap) memcpy(keys, hs.keys, std::min<uint64_t>(hs.nkeys, cap) * sizeof(uint64_t));
+    return (int64_t)hs.nkeys;
 }
 
 // krep.c:1873-1914

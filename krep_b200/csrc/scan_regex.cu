@@ -17,7 +17,9 @@
 //   * in count mode (fused -E -c) the same walk counts the lines it decides MATCHED (one atomic per warp) and emits
 //     keys for the uncertain lines only;
 //   * in match mode (offsets on the device) the same walk decides the lines, and each line decided MATCHED is walked
-//     again with the anchored match automaton to emit one key per match, in the reference's order (DESIGN §12.2).
+//     again with the anchored match automaton to emit one key per match, in the reference's order (DESIGN §12.2);
+//   * in batch mode (krep_b200_regex_search_batch) the text is many texts packed with '\n' gaps, and each line belongs
+//     to its own text: gap lines are skipped, each text's last line is uncertain, -c counts per text (DESIGN §12.5).
 //
 // Work per byte: one class lookup and one transition lookup in shared memory.
 #include <cooperative_groups.h>
@@ -112,6 +114,18 @@ enum RxMode : int
     RX_MATCH = 2,  // offsets: one key per match of a line decided MATCHED, uncertain lines leave keys
 };
 
+// Batch count mode: adds the thread's lines of text t to that text's counter.
+template <int MODE>
+__device__ __forceinline__ void add_text_lines(const RegexLaunch &a, uint32_t t, uint32_t &counted)
+{
+    if constexpr (MODE == RX_COUNT)
+        if (counted)
+        {
+            atomicAdd(a.text_lines + t, (unsigned long long)counted);
+            counted = 0;
+        }
+}
+
 // RX_FILTER: the filter (one key per flagged line).  RX_COUNT: the fused -c of plans whose per-line answer is exact
 // (RegexDfa::count_exact).  A line the walk decides (MATCHED or DEAD, or its '\n' read through the '\n' column) is
 // settled on the device, and a MATCHED one is counted; only the uncertain lines leave as keys: a line whose '\n' lies
@@ -119,7 +133,12 @@ enum RxMode : int
 // quirks of the reference stay with glibc: DESIGN §12.1).  RX_MATCH (RegexDfa::offsets_exact): the same uncertain
 // lines leave keys (REGEX_MATCH_SHIFT layout); a line decided MATCHED is enumerated with the anchored match automaton
 // (DESIGN §12.2) within a step budget, and a line over its budget leaves an uncertain key as well.
-template <int MODE>
+// BATCH (krep_b200_regex_search_batch, DESIGN §12.5): the text is many texts packed with '\n' gaps.  Three rules differ:
+// a line that starts in a gap belongs to no text (the walk jumps to the next text's first byte, and processes that line
+// only if it still lies in the segment); in count and match mode the uncertain line is the one holding its own text's
+// last byte (its '\n' is the text's final byte or the gap's first); and count mode adds its lines to one counter per
+// text, once when the thread leaves a text and once at the end.
+template <int MODE, bool BATCH>
 __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constant__ RegexLaunch a)
 {
     extern __shared__ uint4 s_raw[];
@@ -137,7 +156,10 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
     const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
     const uint64_t nseg = (own + RX_SEG - 1) / RX_SEG;
     Window W{a.text, a.avail_len, ~0ull, make_uint4(0, 0, 0, 0)};
-    uint32_t counted = 0; // RX_COUNT: lines of this thread decided MATCHED
+    uint32_t counted = 0; // RX_COUNT: lines of this thread decided MATCHED (BATCH: of text t, not yet added)
+    // BATCH: the text of the current line start and its global end
+    uint32_t t = 0;
+    uint64_t t_end = 0;
     for (uint64_t sg = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; sg < nseg; sg += (uint64_t)gridDim.x * blockDim.x)
     {
         const uint64_t sb = a.own_begin + sg * RX_SEG;
@@ -150,8 +172,36 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
             p = next_newline(W, sb, se) + 1; // the line in progress belongs to an earlier segment
             if (p > se) continue;
         }
+        if constexpr (BATCH)
+        {
+            const uint32_t t0 = a.seg_text[(a.global_offset + sb) / RX_SEG];
+            if (t0 != t) add_text_lines<MODE>(a, t, counted);
+            t = t0;
+            t_end = 0; // reloaded at the first line
+        }
         while (p < se)
         {
+            if constexpr (BATCH)
+            {
+                // the text this line starts in: texts ending at or before it are behind the thread for good
+                const uint64_t gp = a.global_offset + p;
+                if (gp >= t_end)
+                {
+                    while (t < a.n_texts && (t_end = a.text_end[t]) <= gp)
+                    {
+                        add_text_lines<MODE>(a, t, counted);
+                        t++;
+                    }
+                    if (t >= a.n_texts) break; // only the gap after the last text is left
+                    const uint64_t t_start = a.text_start[t];
+                    if (gp < t_start)
+                    {
+                        // a line in the gap: on to the text's first byte (the byte before it is a gap '\n')
+                        p = t_start - a.global_offset;
+                        if (p >= se) break;
+                    }
+                }
+            }
             uint32_t row = a.start;
             uint64_t q = p;
             while (row > dead && q < limit)
@@ -166,7 +216,8 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
             {
                 if (row > dead && q < limit) row = s_tab[row + nl]; // the walk stopped at the line's '\n'
                 if (row <= dead) q = next_newline(W, q, limit);
-                flag = q >= limit || (q + 1 == a.avail_len && a.next_byte < 0); // '\n' out of reach, or the text's last byte
+                if constexpr (BATCH) flag = q >= limit || a.global_offset + q + 1 >= t_end; // out of reach, or its text's last byte
+                else flag = q >= limit || (q + 1 == a.avail_len && a.next_byte < 0); // '\n' out of reach, or the text's last byte
                 if constexpr (MODE == RX_COUNT) counted += (!flag && row == 0) ? 1u : 0u;
             }
             else
@@ -223,7 +274,9 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
             p = q + 1;
         }
     }
-    if constexpr (MODE == RX_COUNT)
+    if constexpr (BATCH)
+        add_text_lines<MODE>(a, t, counted);
+    else if constexpr (MODE == RX_COUNT)
     {
         // every thread of the block gets here: one atomic per warp
         const uint32_t w = __reduce_add_sync(0xFFFFFFFFu, counted);
@@ -233,12 +286,12 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
 
 } // namespace
 
-template <int MODE>
+template <int MODE, bool BATCH>
 static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
     const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256 + (MODE == RX_MATCH ? (size_t)regex_tab_words(a.nmtrans) * 2 : 0);
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE, BATCH>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
     {
         cudaGetLastError();
         per_sm = 1;
@@ -247,17 +300,23 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
     const uint64_t blocks_needed = (own + (uint64_t)RX_SEG * RX_THREADS - 1) / ((uint64_t)RX_SEG * RX_THREADS);
     const uint64_t resident = (uint64_t)sm_count * per_sm;
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
-    trace("regex%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory",
+    trace("regex%s%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", BATCH ? " batch" : "",
           MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", grid, RX_THREADS, per_sm, smem);
-    k_regex_lines<MODE><<<grid, RX_THREADS, smem, s>>>(a);
+    k_regex_lines<MODE, BATCH><<<grid, RX_THREADS, smem, s>>>(a);
     count_launch();
 }
 
 void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
-    if (a.line_count) launch_regex_t<RX_COUNT>(a, sm_count, s);
-    else if (a.matches) launch_regex_t<RX_MATCH>(a, sm_count, s);
-    else launch_regex_t<RX_FILTER>(a, sm_count, s);
+    if (a.text_end)
+    {
+        if (a.text_lines) launch_regex_t<RX_COUNT, true>(a, sm_count, s);
+        else if (a.matches) launch_regex_t<RX_MATCH, true>(a, sm_count, s);
+        else launch_regex_t<RX_FILTER, true>(a, sm_count, s);
+    }
+    else if (a.line_count) launch_regex_t<RX_COUNT, false>(a, sm_count, s);
+    else if (a.matches) launch_regex_t<RX_MATCH, false>(a, sm_count, s);
+    else launch_regex_t<RX_FILTER, false>(a, sm_count, s);
 }
 
 } // namespace kb

@@ -84,6 +84,15 @@ def load():
     L.krep_b200_search_batch.argtypes = [C.c_void_p, C.POINTER(SearchParams), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t,
                                          C.POINTER(C.c_uint64), C.POINTER(C.POINTER(MatchResult))]
     L.krep_b200_search_batch.restype = C.c_int
+    L.krep_b200_regex_search_batch.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t,
+                                               C.POINTER(C.c_uint64), C.POINTER(C.POINTER(MatchResult))]
+    L.krep_b200_regex_search_batch.restype = C.c_int
+    L.krep_b200_regex_batch_stats.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    L.krep_b200_regex_batch_stats.restype = None
+    L.krep_b200_regex_search_batch_raw.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_size_t,
+                                                   C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_uint64,
+                                                   C.POINTER(C.c_uint64)]
+    L.krep_b200_regex_search_batch_raw.restype = C.c_int64
     L.krep_b200_scan_shard_begin.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.c_void_p, C.POINTER(C.c_int)]
     L.krep_b200_scan_shard_begin.restype = C.c_int
     L.krep_b200_scan_shard_end.argtypes = [C.c_int, C.POINTER(DeviceResult)]
@@ -232,6 +241,33 @@ def search_batch(func, params, texts, with_result=True):
             L.krep_b200_ac_trie_free(params.struct.ac_trie)
             params.struct.ac_trie = None
         L.krep_b200_set_only_matching(False)
+
+
+def text_array(texts):
+    """(keep-alive buffers, char* array, size_t array) for a list of bytes objects."""
+    n = len(texts)
+    bufs = [C.create_string_buffer(t, max(len(t), 1)) for t in texts]
+    tarr = (C.c_char_p * max(n, 1))(*[C.cast(b, C.c_char_p) for b in bufs])
+    larr = (C.c_size_t * max(n, 1))(*[len(t) for t in texts])
+    return bufs, tarr, larr
+
+
+def regex_search_batch(params, texts, with_result=True):
+    """krep_b200_regex_search_batch on a list of bytes objects. -> [(count, [(start, end), ...]), ...]"""
+    L = load()
+    n = len(texts)
+    _bufs, tarr, larr = text_array(texts)
+    counts = (C.c_uint64 * max(n, 1))()
+    res = [L.krep_b200_match_result_init(16) for _ in range(n)] if with_result else []
+    rarr = (C.POINTER(MatchResult) * max(n, 1))(*res) if with_result else None
+    try:
+        rc = L.krep_b200_regex_search_batch(params.ref(), tarr, larr, n, counts, rarr)
+        check(L)
+        assert rc == 0, rc
+        return [(int(counts[i]), _positions(res[i]) if with_result else []) for i in range(n)]
+    finally:
+        for r in res:
+            L.krep_b200_match_result_free(r)
 
 
 def _positions(res):
