@@ -524,14 +524,10 @@ int launch_count_lines(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh,
         D.exact = (window && plan->m <= 4 && plan->whole_word == 0 && (plan->case_sensitive || letters)) ? 1u : 0u;
     }
     const uint64_t groups = p.group_end - p.group_begin;
-    static uint32_t part_default = 0;
-    if (!part_default)
-    {
-        const char *v = getenv("KREP_B200_COUNT_PART_KB");
-        uint32_t kb_ = v && atoi(v) > 0 ? (uint32_t)atoi(v) : 64;
-        part_default = std::max<uint32_t>(128, kb_ * 64 / 128 * 128); // groups, a multiple of the 128-group tile
-    }
-    uint64_t part = part_default;
+    // read on every launch (getenv is nothing next to a launch), so that a process can change the partition size
+    const char *v = getenv("KREP_B200_COUNT_PART_KB");
+    const uint32_t kb_ = v && atoi(v) > 0 ? (uint32_t)atoi(v) : 64;
+    uint64_t part = std::max<uint32_t>(128, kb_ * 64 / 128 * 128); // groups, a multiple of the 128-group tile
     const uint64_t max_parts = 1u << 18;
     if ((groups + part - 1) / part > max_parts) part = ((groups + max_parts - 1) / max_parts + 127) / 128 * 128;
     D.part_groups = (uint32_t)part;

@@ -97,8 +97,8 @@ def test_port_matches_committed_reference_fixtures():
 ALPHABETS = [b"ab", b"abc \n", b"aAbB_ 1\n", b"abcdefghij klmnop\nQRS"]
 
 
-def random_case(rng, func):
-    alpha = rng.choice(ALPHABETS)
+def random_case(rng, func, alphabets=ALPHABETS):
+    alpha = rng.choice(alphabets)
     n = rng.choice([0, 1, 2, 3, 5, 8, 15, 16, 17, 31, 33, 64, 100, 257, 1000])
     text = bytes(rng.choice(alpha) for _ in range(n))
     if func == "aho_corasick":

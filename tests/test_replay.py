@@ -11,61 +11,11 @@ import oracle_util as ou
 from krep_b200 import lib
 from krep_b200.abi import (ALGO_AC, ALGO_AVX2, ALGO_AVX512, ALGO_BMH, ALGO_KMP, ALGO_MEMCHR, ALGO_MEMCHR_SHORT, ALGO_NEON,
                            ALGO_SSE42, MatchResult, Params, SIZE_MAX)
+from scan_model import device_like_keys
 from test_oracle import random_case
 
 ALGO = {"boyer_moore": ALGO_BMH, "kmp": ALGO_KMP, "memchr": ALGO_MEMCHR, "memchr_short": ALGO_MEMCHR_SHORT,
         "sse42": ALGO_SSE42, "aho_corasick": ALGO_AC, "avx2": ALGO_AVX2, "avx512": ALGO_AVX512, "neon": ALGO_NEON}
-
-
-def lc(b):
-    return b.lower()
-
-
-def wordc(c):
-    return chr(c).isascii() and (chr(c).isalnum() or c == 0x5F)
-
-
-def ww_ok(text, s, e):
-    return not ((s > 0 and wordc(text[s - 1])) or (e < len(text) and wordc(text[e])))
-
-
-def ww_tag(text, s, e):
-    """ws_ok << 1 | we_ok — the two halves of is_whole_word_match as the device tags them (csrc/common.h)."""
-    return (0 if (s > 0 and wordc(text[s - 1])) else 2) | (0 if (e < len(text) and wordc(text[e])) else 1)
-
-
-def device_like_keys(func, pats, text, cs, whole_word, only_matching):
-    """What the device list contains for this call (tag mode: every occurrence, ww bit set per key)."""
-    keys = []
-    if func == "aho_corasick":
-        for k, p in enumerate(pats):
-            if not p:
-                continue
-            pp, tt = (p, text) if cs else (lc(p), lc(text))
-            s = tt.find(pp)
-            while s >= 0:
-                if not whole_word or ww_ok(text, s, s + len(p)):
-                    keys.append(((s + len(p)) << 24) | ((1023 - (len(p) - 1)) << 14) | k)
-                s = tt.find(pp, s + 1)
-        return sorted(keys)
-    p = pats[0]
-    if func == "memchr":
-        p = p[:1]
-    m = len(p)
-    pp, tt = (p, text) if cs else (lc(p), lc(text))
-    prefix_mode = func == "memchr_short" and only_matching
-    for s in range(len(text)):
-        if prefix_mode:
-            if tt[s:s + 1] != pp[:1]:
-                continue
-            full = tt[s:s + m] == pp
-        else:
-            if tt[s:s + m] != pp or s + m > len(text):
-                continue
-            full = True
-        tag = ww_tag(text, s, s + m) if whole_word else 3
-        keys.append((s << 3) | (int(full) << 2) | tag)
-    return keys
 
 
 def replay(func, params, keys, text, with_result):
