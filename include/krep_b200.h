@@ -378,8 +378,8 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan, const search_params_t *
 uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan, const search_params_t *params,
                                  const krep_b200_shard_t *shards, uint32_t n_shards, match_result_t *result);
 
-/* -E over resident shards in two steps, so that one code path serves one process and a multi-rank gather (each rank
- * exports its shards' rows, one variable-length gather brings them to one host, which resolves).
+/* -E over resident shards in two steps, so that one code path serves one process and several ranks (each rank exports
+ * its shard's row and resolves its own lines with krep_b200_regex_resolve_part below; rank 0 gathers the answers).
  * krep_b200_regex_export_shard: one k_regex_lines scan of the shard in the mode krep_b200_regex_search would use for
  * params, then the pack kernels: the shard's row (layout: csrc/common.h, RegexRowHeader) in engine-owned device memory
  * of the shard's device — *d_row (may be NULL), valid until the next export on that device — and *row_bytes.  When dst
@@ -390,6 +390,40 @@ int krep_b200_regex_export_shard(const krep_b200_plan_t *plan, const search_para
 /* The answer of the search from the rows (host memory, text order) of shards that tile the text: what
  * krep_b200_search_shards returns.  Host only; 0 with error -3 when the rows are not rows of one tiling. */
 uint64_t krep_b200_regex_resolve(const search_params_t *params, const void *const *rows, uint32_t n_rows, match_result_t *result);
+/* -E over shards resident on several ranks (one process per GPU, krep_b200/sharding.py; DESIGN §12.6): each rank resolves
+ * the lines its own shard owns, and only counts and positions travel.
+ * krep_b200_regex_resolve_part: the answer of the lines owned by rows[0 .. n_own) — consecutive shards of one tiling of
+ * a text of text_len bytes whose last byte is last_byte (-1 when empty) — capped at params->max_count.
+ * rows[n_own .. n_rows) are the shards that follow, in order; only their heads are read (full rows or head-only rows).
+ * decides_end: this part decides the end of the text (the empty string at text_len); exactly one part of a tiling does,
+ * the owner of the last line start (krep_b200_regex_tiling's decider).  Each part's answer is the first max_count items
+ * of its unbounded answer, so the search's answer is the parts' positions concatenated in text order and cut to
+ * max_count, with count min(sum of counts, max_count).  krep_b200_regex_resolve is the case n_own == n_rows,
+ * decides_end = 1.  Same early returns as krep_b200_regex_resolve; 0 with error -3 when the rows are not consecutive
+ * shards of such a text or a line the part owns runs past the heads it is given. */
+uint64_t krep_b200_regex_resolve_part(const search_params_t *params, const void *const *rows, uint32_t n_rows, uint32_t n_own,
+                                      uint64_t text_len, int last_byte, int decides_end, match_result_t *result);
+/* A head-only row: the row's header with nkeys = nseg = 0, followed by its head.  Returns its size, or the size needed
+ * (nothing copied) when dst is NULL or cap is too small; 0 with error -3 when row is not a regex row. */
+uint64_t krep_b200_regex_row_head(const void *row, void *dst, uint64_t cap);
+/* A row's header: its first KREP_B200_REGEX_ROW_HEADER bytes, all that krep_b200_regex_tiling reads. */
+#define KREP_B200_REGEX_ROW_HEADER 128
+typedef struct
+{
+   uint64_t text_len;  /* the text the rows tile                                                                  */
+   int32_t last_byte;  /* its last byte, -1 when it is empty                                                      */
+   uint32_t decider;   /* the shard that decides the end of the text: the last one that holds a line start (0 for
+                          the empty text)                                                                         */
+} krep_b200_regex_tiling_t;
+/* The geometry of n rows' headers (shard i's at i * KREP_B200_REGEX_ROW_HEADER bytes, text order): whether they tile
+ * one text — the first owns from 0 at a line start, owned ranges abut, the last ends the text, and only empty shards
+ * follow a shard that ends it — and which part reads which head.  A shard holds a line start when it is not empty and
+ * either starts at one (no head) or its head ends before its owned range does.  head_to[i] (may be NULL): the shard
+ * whose part reads shard i's head — the last earlier shard that holds a line start, the owner of the line shard i's
+ * head continues — or -1 when shard i has no head; head_bytes[i] (may be NULL): the size of shard i's head-only row
+ * (krep_b200_regex_row_head), 0 when it sends none.  Returns 0, or -3 when the rows do not tile one text. */
+int krep_b200_regex_tiling(const void *headers, uint32_t n, krep_b200_regex_tiling_t *out, int32_t *head_to,
+                           uint64_t *head_bytes);
 /* Timing of the most recent krep_b200_search_shards (regex plan) or krep_b200_regex_export_shard call on this thread,
  * summed over its shards: device ms of the scans (with their sort) and of the pack kernels, and the row bytes. */
 void krep_b200_regex_export_stats(float *scan_ms, float *pack_ms, uint64_t *packed_bytes);

@@ -65,6 +65,13 @@ class DeviceResult(C.Structure):  # krep_b200_device_result_t
     ]
 
 
+REGEX_ROW_HEADER = 128  # KREP_B200_REGEX_ROW_HEADER
+
+
+class RegexTiling(C.Structure):  # krep_b200_regex_tiling_t
+    _fields_ = [("text_len", C.c_uint64), ("last_byte", C.c_int32), ("decider", C.c_uint32)]
+
+
 class CorpusSpec(C.Structure):  # krep_b200_corpus_spec_t
     _fields_ = [
         ("seed", C.c_uint64),

@@ -7,7 +7,8 @@ usable every search call reports an error through krep_b200_last_error().
 import ctypes as C
 import os
 
-from .abi import (CorpusSpec, DeviceResult, MatchResult, Params, SearchParams, Shard, SEARCH_FUNC, SIZE_MAX)  # noqa: F401
+from .abi import (REGEX_ROW_HEADER, CorpusSpec, DeviceResult, MatchResult, Params, RegexTiling, SearchParams, Shard,  # noqa: F401
+                  SEARCH_FUNC, SIZE_MAX)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KREP_B200_LIB") or os.path.join(_HERE, "libkrep_b200.so")  # override: kernel-variant builds
@@ -128,6 +129,14 @@ def load():
     L.krep_b200_regex_export_shard.restype = C.c_int
     L.krep_b200_regex_resolve.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(MatchResult)]
     L.krep_b200_regex_resolve.restype = C.c_uint64
+    L.krep_b200_regex_resolve_part.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, C.c_uint64,
+                                               C.c_int, C.c_int, C.POINTER(MatchResult)]
+    L.krep_b200_regex_resolve_part.restype = C.c_uint64
+    L.krep_b200_regex_row_head.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+    L.krep_b200_regex_row_head.restype = C.c_uint64
+    L.krep_b200_regex_tiling.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(RegexTiling), C.POINTER(C.c_int32),
+                                         C.POINTER(C.c_uint64)]
+    L.krep_b200_regex_tiling.restype = C.c_int
     L.krep_b200_regex_export_stats.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_uint64)]
     L.krep_b200_last_kernel_ms.restype = C.c_float
     L.krep_b200_launch_count.restype = C.c_uint64
@@ -302,3 +311,46 @@ def regex_resolve(params, rows, with_result=True):
     finally:
         if res:
             L.krep_b200_match_result_free(res)
+
+
+def regex_resolve_part(params, rows, n_own, text_len, last_byte, decides_end, with_result=True):
+    """krep_b200_regex_resolve_part over host rows (bytes-like objects, text order): the answer of the lines rows[:n_own]
+    own. -> (count, [(start, end), ...])"""
+    L = load()
+    bufs = [C.create_string_buffer(bytes(r), max(len(r), 1)) for r in rows]
+    arr = (C.c_void_p * max(len(rows), 1))(*[C.cast(b, C.c_void_p) for b in bufs])
+    res = L.krep_b200_match_result_init(16) if with_result else None
+    try:
+        cnt = L.krep_b200_regex_resolve_part(params.ref(), arr, len(rows), n_own, text_len, last_byte, int(decides_end), res)
+        check(L)
+        return int(cnt), (_positions(res) if res else [])
+    finally:
+        if res:
+            L.krep_b200_match_result_free(res)
+
+
+def regex_row_head(row):
+    """krep_b200_regex_row_head: the head-only row of a row (bytes-like). -> bytes"""
+    L = load()
+    src = C.create_string_buffer(bytes(row), max(len(row), 1))
+    n = L.krep_b200_regex_row_head(src, None, 0)
+    check(L)
+    dst = C.create_string_buffer(n)
+    assert L.krep_b200_regex_row_head(src, dst, n) == n
+    return dst.raw
+
+
+def regex_tiling(headers, n):
+    """krep_b200_regex_tiling over n row headers packed in `headers` (a buffer address or bytes-like).
+    -> (RegexTiling, head_to list, head_bytes list); raises RuntimeError when the rows do not tile one text."""
+    L = load()
+    if not isinstance(headers, int):
+        keep = C.create_string_buffer(bytes(headers), max(len(headers), 1))
+        headers = C.addressof(keep)
+    out = RegexTiling()
+    to = (C.c_int32 * n)()
+    nb = (C.c_uint64 * n)()
+    rc = L.krep_b200_regex_tiling(C.c_void_p(headers), n, C.byref(out), to, nb)
+    if rc != 0:
+        raise RuntimeError("krep_b200: " + L.krep_b200_last_error_string().decode())
+    return out, list(to), list(nb)

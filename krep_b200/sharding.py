@@ -13,6 +13,9 @@ by key (krep_b200_merge_keys, C); the disorder is confined to max_pattern_len by
 one linear pass per cut.
 
 Works on any torch.distributed backend (nccl on the GPUs, gloo in the CPU tests).
+
+-E plans take another exchange (regex_resolve_ranks, RegexRanks; DESIGN §12.6): each rank resolves the lines its own
+shard owns from its own row, and only counts and positions travel to rank 0.
 """
 import ctypes as C
 
@@ -142,3 +145,143 @@ class KeyGatherer:
             self.overflowed = True
             counts = [min(c, self.cap) for c in counts]
         return merge_rows(rows, counts, self.merged), counts
+
+
+# ---- -E over rank-resident shards (DESIGN §12.6) ----
+
+def _result_positions(res):
+    """The positions of a match_result_t as an int64 [k, 2] CPU tensor (one copy, no per-position Python)."""
+    import numpy as np
+    r = res.contents
+    if r.count == 0:
+        return torch.zeros((0, 2), dtype=torch.int64)
+    flat = np.ctypeslib.as_array(C.cast(r.positions, C.POINTER(C.c_uint64)), shape=(2 * r.count,))
+    return torch.from_numpy(flat.astype(np.int64)).view(-1, 2)
+
+
+def regex_resolve_ranks(params, row, rank, world, device="cpu", group=None, times=None):
+    """One -E answer from rows spread over the ranks: every rank passes its own shard's row and resolves the lines that
+    shard owns; only counts and positions travel to rank 0.
+
+    row: this rank's row (krep_b200_regex_export_shard) in a uint8 CPU tensor (it may be longer than the row).  The
+    shards of ranks 0 .. world-1 must tile one text in rank order.  device: where the collectives' tensors live — "cpu"
+    for gloo, the rank's CUDA device for NCCL.  times (a dict, optional) receives exchange_ms and resolve_ms.
+    Returns (count, positions as an int64 [k, 2] tensor in the reference's order) on rank 0, None elsewhere.
+
+      1. one all_gather of the 128-byte row headers: from them every rank knows the tiling, the text's last byte, which
+         rank decides the end of the text, and which heads it receives (krep_b200_regex_tiling).  A tiling error is
+         raised on every rank alike, before any further collective, so none is left waiting;
+      2. every shard that starts mid-line sends its head-only row (krep_b200_regex_row_head) to the rank that owns the
+         line it continues, point to point (the sizes are known from the headers);
+      3. every rank resolves its part (krep_b200_regex_resolve_part) with the full -m budget;
+      4. one all_gather of (count, positions), then the positions are gathered to rank 0, which concatenates them in
+         rank order and cuts them to max_count: each part's answer is the first max_count items of its own unbounded
+         answer, so this is the whole answer."""
+    import time
+    L = lib.load()
+    t0 = time.perf_counter()
+    hb = lib.REGEX_ROW_HEADER
+    mine = row[:hb].to(device)
+    heads = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(heads, mine, group=group)
+    headers = torch.cat([h.cpu() for h in heads]).contiguous()
+    tiling, head_to, head_bytes = lib.regex_tiling(headers.data_ptr(), world)
+    ops, recv = [], []
+    if head_to[rank] >= 0:
+        out = torch.empty(head_bytes[rank], dtype=torch.uint8)
+        n = L.krep_b200_regex_row_head(C.c_void_p(row.data_ptr()), C.c_void_p(out.data_ptr()), out.numel())
+        lib.check(L)
+        assert n == out.numel(), (n, out.numel())
+        ops.append(dist.isend(out.to(device), head_to[rank], group=group))
+    for j in range(world):
+        if head_to[j] == rank:
+            buf = torch.empty(head_bytes[j], dtype=torch.uint8, device=device)
+            recv.append(buf)
+            ops.append(dist.irecv(buf, j, group=group))
+    for op in ops:
+        op.wait()
+    rows = [row] + [b.cpu() for b in recv]  # the heads of the shards after this one, in text order
+    t1 = time.perf_counter()
+    arr = (C.c_void_p * len(rows))(*[r.data_ptr() for r in rows])
+    res = L.krep_b200_match_result_init(16)
+    try:
+        cnt = L.krep_b200_regex_resolve_part(params.ref(), arr, len(rows), 1, tiling.text_len, tiling.last_byte,
+                                             int(tiling.decider == rank), res)
+        err = L.krep_b200_last_error()
+        msg = L.krep_b200_last_error_string().decode() if err else ""
+        pos = _result_positions(res)
+    finally:
+        L.krep_b200_match_result_free(res)
+    t2 = time.perf_counter()
+    # an error of one part travels with the counts, so every rank raises it and none waits in the gather below
+    meta = torch.tensor([int(cnt), pos.shape[0], err], dtype=torch.int64, device=device)
+    metas = [torch.empty_like(meta) for _ in range(world)]
+    dist.all_gather(metas, meta, group=group)
+    metas = torch.stack([m.cpu() for m in metas])
+    bad = [r for r in range(world) if metas[r, 2] != 0]
+    if bad:
+        raise RuntimeError(f"krep_b200_regex_resolve_part failed on rank(s) {bad}" + (f": {msg}" if msg else ""))
+    counts, npos = metas[:, 0].tolist(), metas[:, 1].tolist()
+    mx = max(npos)
+    parts = [pos]
+    if mx:
+        padded = torch.zeros((mx, 2), dtype=torch.int64, device=device)
+        padded[:pos.shape[0]] = pos.to(device)
+        got = [torch.empty_like(padded) for _ in range(world)] if rank == 0 else None
+        dist.gather(padded, got, dst=0, group=group)
+        if rank == 0:
+            parts = [g[:k].cpu() for g, k in zip(got, npos)]
+    t3 = time.perf_counter()
+    if times is not None:
+        times["exchange_ms"] = ((t1 - t0) + (t3 - t2)) * 1e3
+        times["resolve_ms"] = (t2 - t1) * 1e3
+    if rank != 0:
+        return None
+    max_count = int(params.struct.max_count)
+    return min(sum(counts), max_count), torch.cat(parts)[:max_count]
+
+
+class RegexRanks:
+    """-E search of this rank's resident shard as one part of a text tiled across the ranks: the export into a
+    persistent host buffer (grown when a row does not fit), then regex_resolve_ranks.  The row, the heads and the
+    answers live on the host, so a gloo group is the natural transport; bench_regex_ranks.py uses one.  NCCL works too
+    (device = the rank's GPU): every message is then staged through it."""
+
+    def __init__(self, rank, world, device="cpu", group=None, capacity=1 << 20):
+        self.rank, self.world, self.device, self.group = rank, world, device, group
+        self.row = torch.empty(capacity, dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+        self.times = {}
+
+    def export(self, plan, params, shard):
+        """This rank's row into self.row; -> its size in bytes."""
+        import time
+        L = lib.load()
+        t0 = time.perf_counter()
+        nb = C.c_uint64(0)
+        rc = L.krep_b200_regex_export_shard(plan, params.ref(), C.byref(shard), None, C.c_void_p(self.row.data_ptr()),
+                                            self.row.numel(), C.byref(nb), None)
+        if rc == -5:  # the row needs more room: grow and export again
+            L.krep_b200_last_error()
+            self.row = torch.empty(nb.value + nb.value // 4, dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+            rc = L.krep_b200_regex_export_shard(plan, params.ref(), C.byref(shard), None, C.c_void_p(self.row.data_ptr()),
+                                                self.row.numel(), C.byref(nb), None)
+        if rc != 0:
+            raise RuntimeError("krep_b200: " + L.krep_b200_last_error_string().decode())
+        self.times["export_ms"] = (time.perf_counter() - t0) * 1e3
+        return nb.value
+
+    def search(self, plan, params, shard):
+        """-> (count, int64 [k, 2] positions) on rank 0, None elsewhere.
+
+        Every rank must call it with the same plan and params.  An export that fails on one rank (a refused pattern, a
+        CUDA error) still takes part in the exchange with a header no tiling accepts, so every rank raises."""
+        try:
+            self.export(plan, params, shard)
+        except RuntimeError:
+            self.row[:lib.REGEX_ROW_HEADER].zero_()
+            try:
+                regex_resolve_ranks(params, self.row, self.rank, self.world, self.device, self.group)
+            except RuntimeError:
+                pass
+            raise
+        return regex_resolve_ranks(params, self.row, self.rank, self.world, self.device, self.group, self.times)
