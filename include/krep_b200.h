@@ -159,7 +159,12 @@ uint64_t krep_b200_neon_search(const search_params_t *, const char *, size_t, ma
  * Refused (the pattern stays with the host's regex_search): back-references, \` \', \s \S \W, [[:space:]],
  * [[:cntrl:]], collating elements, any character set that holds '\n' or a newline in the pattern, non-ASCII pattern
  * bytes, unknown escapes, a process running in a multibyte locale (krep itself never calls setlocale), and automata
- * above 4096 states or 32 KiB of transition table. */
+ * above 4096 states or 32 KiB of transition table (or 8192 NFA states, or 255 byte classes).  A regex whose top level
+ * is an alternation (krep's (p1)|...|(pk) of several -e or -f patterns, or one pattern with a top-level |) and whose
+ * one automaton is too large is split instead: its branches, in order, go to up to 8 automata that the scan walks
+ * together (a split plan).  The size refusal then applies to a single branch that no automaton holds, and to sets whose
+ * automata need more than 224 KiB of shared memory together (about 500 patterns of 8-12 lowercase letters); a split
+ * plan computes offsets on the GPU only when its match automata fit in the same 224 KiB as well. */
 uint64_t krep_b200_regex_search(const search_params_t *, const char *, size_t, match_result_t *);
 
 /* Many texts, one launch — what search_directory_recursive (krep.c:3310) calling search_file once per small file
@@ -474,6 +479,21 @@ int64_t krep_b200_regex_matches_host(const search_params_t *params, const char *
  * No search entry point calls it. */
 int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
                                        uint64_t *keys, uint64_t cap, uint64_t *device_lines);
+/* Test hook: how many automata the -E plan of params has — G >= 2 for a split plan (see krep_b200_regex_search), 1 for
+ * a plan of one automaton, -1 when the pattern is refused. */
+int krep_b200_regex_automata(const search_params_t *params);
+/* Test hook: a -E plan of params compiled with a cap of max_states (3 .. 4096) states per automaton instead of 4096,
+ * so that small regexes with a top-level alternation become split plans.  The plan is not cached and no search entry
+ * point uses it; scan it with krep_b200_regex_scan_shard_raw, run it with krep_b200_regex_plan_host, and free it with
+ * krep_b200_plan_destroy.  NULL (error -3) when the regex is refused under that cap. */
+krep_b200_plan_t *krep_b200_regex_plan_split(const search_params_t *params, uint32_t max_states);
+/* Test hook, host only: the host twin of one krep_b200_regex_scan_shard_raw scan of the whole `text` (one shard from
+ * offset 0, nothing after it) with `plan`, every line walked at most `reach` bytes (UINT64_MAX: no bound) in modes 1
+ * and 2; mode 0 has no bound.  Keys, in the layout of the mode, sorted, go to keys[0 .. min(result, cap)) and
+ * *device_lines (may be NULL) gets the count mode's lines decided MATCHED.  Returns the number of keys, or -3 when the
+ * plan does not admit the mode. */
+int64_t krep_b200_regex_plan_host(const krep_b200_plan_t *plan, int mode, const char *text, size_t n, uint64_t reach,
+                                  uint64_t *keys, uint64_t cap, uint64_t *device_lines);
 /* Test hook: one batch scan of krep_b200_regex_search_batch in `mode` (0, 1, 2 as above) over the texts with lens[i] > 0.
  * offsets[i] (may be NULL): text i's packed offset (UINT64_MAX for a text not packed); keys[0 .. min(result, cap)):
  * the sorted keys in packed coordinates; text_lines[i] (may be NULL): in mode 1 the lines of text i decided MATCHED on

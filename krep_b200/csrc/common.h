@@ -97,12 +97,39 @@ struct RegexDfa
     bool offsets_exact = false;
     std::vector<uint16_t> match;
     uint32_t match_bol = 0, match_mid = 0;
+    // A split plan (DESIGN §12.7) holds the automata of its groups here, each compiled as a regex of its own, and only
+    // the three flags above (the union's); a plan of one automaton leaves it empty.
+    std::vector<RegexDfa> groups;
 };
 static constexpr uint16_t RX_ACC = 1, RX_ACC_EOL = 2;
 // Padded size in 16-bit words of the table image the kernel copies to shared memory: line table, class map, match table.
 __host__ __device__ inline uint32_t regex_tab_words(uint32_t ntrans) { return (ntrans + 7) & ~7u; }
+
+// Split plans (DESIGN §12.7).  A regex whose one automaton is refused for size, and whose top level is an alternation
+// B1|...|Bk (krep's (p1)|...|(pk) of -f / several -e), is compiled as up to REGEX_MAX_GROUPS automata, one per group
+// of consecutive branches, that k_regex_lines walks together.  The whole image lives in the shared memory of one CTA,
+// at most REGEX_SET_SMEM_BYTES (a constant: plans are built before any device is known; sm_90 lets a block opt in to
+// 227 KiB).  The line tables and class maps must fit, or the plan is refused; offsets stay on the device only when the
+// match tables fit as well.  Measured envelope: 200 lowercase literals of 8-12 bytes fit with offsets (about 95 KiB of
+// line tables and 95 KiB of match tables), 200 alphanumeric ones without (176 KiB of line tables), 500 lowercase ones
+// not at all (235 KiB of line tables).
+static constexpr uint32_t REGEX_MAX_GROUPS = 8;
+static constexpr uint32_t REGEX_SET_SMEM_BYTES = 224 * 1024;
+// One automaton of a plan's image as the kernel reads it: 16-bit word offsets of its line table, class map and match
+// table in the image, and its RegexDfa numbers.
+struct RegexGroup
+{
+    uint32_t trans, cls, match;
+    uint32_t nclasses, nl_class, start, match_bol, match_mid;
+};
+// The image of a plan: every automaton's line table (padded to 16 bytes) and class map, in order, then every match table
+// (padded).  A plan of one automaton gives the layout k_regex_lines reads.  grp[REGEX_MAX_GROUPS]: the automata, and in
+// the slots past *ngroups the first one started DEAD; *line_words: the words the filter and count modes read.
+void regex_layout(const RegexDfa &D, RegexGroup *grp, uint32_t *ngroups, uint32_t *line_words, uint32_t *image_words);
+std::vector<uint16_t> regex_image(const RegexDfa &D);
 bool regex_source(const search_params_t *P, std::string *out); // the string krep compiles (krep.c:2081-2145)
-int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why); // 0, or -1 = refused (*why)
+// 0, or -1 = refused (*why).  max_states: the state cap of each automaton (tests lower it to force split plans).
+int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why, uint32_t max_states = REGEX_MAX_STATES);
 void regex_lines_host(const RegexDfa &D, const char *text, size_t n, std::vector<uint64_t> *line_starts);
 // The count mode of k_regex_lines on the host, every line walked at most `reach` bytes: returns the lines decided
 // MATCHED and stores the uncertain line starts (live at the bound, or holding the text's last byte) in *uncertain.
@@ -172,6 +199,10 @@ struct RegexLaunch
     const uint32_t *seg_text;              // per global 256-byte segment g: the first text i with text_end[i] > g * 256
     unsigned long long *text_lines;        // count mode: lines of text i decided MATCHED (replaces line_count)
     uint32_t n_texts;
+    // split plans (ngroups >= 2): the automata of the image at `trans` (regex_layout); line_words of it are
+    // copied to shared memory in the filter and count modes, image_words in match mode
+    uint32_t ngroups, line_words, image_words;
+    RegexGroup grp[REGEX_MAX_GROUPS];
 };
 static_assert(REGEX_SEG == 256, "RegexLaunch::seg_text has one entry per 256 bytes");
 // The device copies of a batch's text table (RegexLaunch batch fields), handed to launch_scan.
@@ -193,7 +224,7 @@ struct PlanDev
     bool ready = false;
     uint8_t *d_pat_val = nullptr, *d_pat_mask = nullptr; // literal
     AcDevTables *ac = nullptr;                           // pattern set
-    uint16_t *d_regex = nullptr;                         // regex: transition table + class map
+    uint16_t *d_regex = nullptr;                         // regex: the plan's image (regex_layout)
 };
 
 struct Plan
@@ -275,7 +306,7 @@ struct AcLaunch
 void launch_ac(const Plan *plan, const AcDevTables *T, const AcLaunch &a, int sm_count, cudaStream_t s);
 void count_launch(int n = 1);
 // regex kernel (scan_regex.cu)
-void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s);
+int launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s); // 0, or -2 with the error set
 
 // semantics.cpp — reference control flow replayed over the sorted occurrence list
 struct Replay

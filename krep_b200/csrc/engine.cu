@@ -399,14 +399,8 @@ const PlanDev *plan_on_device(const Plan *plan, DevCtx &C)
     }
     else if (plan->is_regex)
     {
-        // transition table, padded to 16 bytes, then the class map, then the match table of an offsets_exact plan (padded
-        // too): k_regex_lines copies what its mode reads to shared memory as vectors
-        const RegexDfa &D = *plan->rx;
-        const size_t tw = regex_tab_words((uint32_t)D.trans.size());
-        std::vector<uint16_t> img(tw + 128 + regex_tab_words((uint32_t)D.match.size()), 0);
-        std::copy(D.trans.begin(), D.trans.end(), img.begin());
-        memcpy(img.data() + tw, D.cls, 256);
-        std::copy(D.match.begin(), D.match.end(), img.begin() + tw + 128);
+        // the plan's image (regex_layout): the kernel copies what its mode reads to shared memory as vectors
+        const std::vector<uint16_t> img = regex_image(*plan->rx);
         if (cudaMalloc(&pd.d_regex, img.size() * 2) != cudaSuccess ||
             cudaMemcpy(pd.d_regex, img.data(), img.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess)
         {
@@ -450,9 +444,10 @@ static bool border_free(const std::string &s, bool cs)
     return pi[m - 1] == 0;
 }
 
-// -E: the line automaton of the regex krep compiled from params->patterns.  nullptr and *why when the compiler refuses
-// the pattern (no error is raised: a refused regex simply stays on the host's regex_search).
-Plan *regex_plan_build(const search_params_t *P, std::string *why)
+// -E: the line automaton of the regex krep compiled from params->patterns (or the automata of a split plan).  nullptr and
+// *why when the compiler refuses the pattern (no error is raised: a refused regex simply stays on the host's
+// regex_search).  max_states: the state cap of each automaton, REGEX_MAX_STATES but for test plans.
+Plan *regex_plan_build(const search_params_t *P, std::string *why, uint32_t max_states)
 {
     std::string re;
     if (!regex_source(P, &re))
@@ -461,7 +456,7 @@ Plan *regex_plan_build(const search_params_t *P, std::string *why)
         return nullptr;
     }
     RegexDfa *D = new RegexDfa();
-    if (regex_compile(re, !P->case_sensitive, D, why) != 0)
+    if (regex_compile(re, !P->case_sensitive, D, why, max_states) != 0)
     {
         delete D;
         return nullptr;
@@ -473,7 +468,7 @@ Plan *regex_plan_build(const search_params_t *P, std::string *why)
     pl->whole_word = P->whole_word ? 1 : 0;
     pl->regex = re;
     pl->rx = D;
-    pl->filter_name = D->widened ? "regex-lines-widened" : "regex-lines";
+    pl->filter_name = std::string(D->groups.empty() ? "regex-lines" : "regex-lines-split") + (D->widened ? "-widened" : "");
     std::lock_guard<std::mutex> lp(g_plans_mu);
     g_all_plans.push_back(pl);
     return pl;
@@ -633,8 +628,8 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.seg_text = regex_batch ? regex_batch->seg_text : nullptr;
         a.text_lines = regex_batch ? regex_lines : nullptr;
         a.n_texts = regex_batch ? regex_batch->n_texts : 0u;
-        launch_regex(a, E.sm_count, stream);
-        return 0;
+        regex_layout(*plan->rx, a.grp, &a.ngroups, &a.line_words, &a.image_words);
+        return launch_regex(a, E.sm_count, stream);
     }
     if (plan->is_ac)
     {

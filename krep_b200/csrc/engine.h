@@ -128,7 +128,8 @@ struct DeviceGuard // restores the calling thread's current device
 };
 
 Plan *plan_build(const search_params_t *P, int algo, bool only_matching);
-Plan *regex_plan_build(const search_params_t *P, std::string *why); // nullptr = refused (no error raised)
+// nullptr = refused (no error raised); max_states below REGEX_MAX_STATES only for test plans (krep_b200_regex_plan_split)
+Plan *regex_plan_build(const search_params_t *P, std::string *why, uint32_t max_states = REGEX_MAX_STATES);
 void plan_free(Plan *p);
 const PlanDev *plan_on_device(const Plan *p, DevCtx &C); // uploads on first use; nullptr on CUDA errors
 int resolve_algo(const search_params_t *P, int algo); // host_api.cu: precondition fallbacks of the simd_* entries

@@ -101,6 +101,16 @@ static Plan *cached_plan(const search_params_t *P, int algo, bool only_matching)
     return pl;
 }
 
+// Regexes the compiler refused (regex string, case flag, reason), most recent last.  Trying to split a large set can
+// take seconds before it is refused, and krep asks once per file (search_file): the refusal is remembered.
+struct RegexRefusal
+{
+    std::string regex;
+    bool case_sensitive;
+    std::string why;
+};
+static std::vector<RegexRefusal> g_regex_refusals;
+
 // The regex plan of params (keyed by the regex string krep compiles and the case flag); nullptr and *why when the
 // compiler refuses the pattern.  Host only: no device is touched until the plan runs.
 static Plan *cached_regex_plan(const search_params_t *P, std::string *why)
@@ -111,6 +121,12 @@ static Plan *cached_regex_plan(const search_params_t *P, std::string *why)
         *why = "no pattern";
         return nullptr;
     }
+    for (const RegexRefusal &r : g_regex_refusals)
+        if (r.case_sensitive == P->case_sensitive && r.regex == re)
+        {
+            *why = r.why;
+            return nullptr;
+        }
     for (size_t i = 0; i < g_plan_cache.size(); i++)
     {
         Plan *pl = g_plan_cache[i];
@@ -123,11 +139,17 @@ static Plan *cached_regex_plan(const search_params_t *P, std::string *why)
     }
     Plan *pl = regex_plan_build(P, why);
     if (pl) cache_insert(pl);
+    else if (MB_CUR_MAX == 1) // a refusal for the process locale may not hold after a setlocale
+    {
+        if (g_regex_refusals.size() >= 16) g_regex_refusals.erase(g_regex_refusals.begin());
+        g_regex_refusals.push_back(RegexRefusal{re, P->case_sensitive, *why});
+    }
     return pl;
 }
 
 void plan_cache_clear()
 {
+    g_regex_refusals.clear();
     for (Plan *p : g_plan_cache) plan_free(p);
     g_plan_cache.clear();
 }
@@ -1915,6 +1937,55 @@ int64_t krep_b200_regex_count_host(const search_params_t *P, const char *text, s
     const uint64_t device_lines = regex_count_lines_host(*pl->rx, text, n, reach, &keys);
     for (uint64_t &k : keys) k <<= LIT_TAG_BITS;
     return (int64_t)regex_count_total(P, device_lines, Replay{keys.data(), keys.size(), text, n, 0});
+}
+
+// ---- test hooks: split plans (DESIGN §12.7) ----
+int krep_b200_regex_automata(const search_params_t *P)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    std::string why;
+    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    if (!pl) return -1;
+    return pl->rx->groups.empty() ? 1 : (int)pl->rx->groups.size();
+}
+
+krep_b200_plan_t *krep_b200_regex_plan_split(const search_params_t *P, uint32_t max_states)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    if (!P || max_states < 3 || max_states > REGEX_MAX_STATES)
+    {
+        set_error(-3, "krep_b200_regex_plan_split: null params, or a state cap outside [3, %u]", REGEX_MAX_STATES);
+        return nullptr;
+    }
+    std::string why;
+    Plan *pl = regex_plan_build(P, &why, max_states); // not in the plan cache: only krep_b200_plan_destroy frees it
+    if (!pl) set_error(-3, "this regex has no plan under a cap of %u states (%s)", max_states, why.c_str());
+    return reinterpret_cast<krep_b200_plan_t *>(pl);
+}
+
+int64_t krep_b200_regex_plan_host(const krep_b200_plan_t *plan_, int mode, const char *text, size_t n, uint64_t reach,
+                                  uint64_t *keys, uint64_t cap, uint64_t *device_lines)
+{
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    const Plan *plan = reinterpret_cast<const Plan *>(plan_);
+    if (!plan || !plan->is_regex || (!text && n) || (cap && !keys) || mode < 0 || mode > 2 ||
+        (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    {
+        set_error(-3, "krep_b200_regex_plan_host: bad argument, or mode %d is not available for this plan", mode);
+        return -3;
+    }
+    std::vector<uint64_t> v;
+    uint64_t lines = 0;
+    if (mode == 0) regex_lines_host(*plan->rx, text, n, &v);
+    else if (mode == 1) lines = regex_count_lines_host(*plan->rx, text, n, reach, &v);
+    else regex_matches_host(*plan->rx, text, n, reach, &v);
+    if (mode != 2)
+        for (uint64_t &k : v) k <<= LIT_TAG_BITS;
+    for (size_t i = 0; i < v.size() && i < cap; i++) keys[i] = v[i];
+    if (device_lines) *device_lines = lines;
+    return (int64_t)v.size();
 }
 
 // ---- test hooks: -E offsets, decided and run on the host ----

@@ -544,25 +544,18 @@ bool regex_source(const search_params_t *P, std::string *out)
     return true;
 }
 
-int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why)
+namespace {
+
+// The automata of the regex rooted at node `root` of a parse: its line automaton and, when its per-line answer is exact,
+// its anchored match automaton.  Every refusal here is one of size (states, table bytes, NFA states, byte classes).
+// parse_widened: the parse widened a set or an assertion.  max_states: REGEX_MAX_STATES, or a smaller test cap.
+// smem_bytes: the shared memory its line table, class map and match table may take together (a split plan checks the
+// sum over its automata afterwards); 0 builds the line automaton only.
+int compile_automaton(const std::vector<Ast> &nodes, int root, bool parse_widened, uint32_t max_states, size_t smem_bytes,
+                      RegexDfa *D, std::string *why)
 {
-    if (MB_CUR_MAX != 1)
-    {
-        // krep never calls setlocale: its regexes are C-locale regexes.  A host running in a multibyte locale compiled
-        // a regex whose '.' and brackets match characters of several bytes, which a byte automaton does not model.
-        *why = "the process runs in a multibyte locale";
-        return -1;
-    }
-    Parser ps(re, icase);
-    int root = ps.parse_alt();
-    if (root >= 0 && ps.i != re.size()) root = ps.refuse("unmatched ')'");
-    if (root < 0)
-    {
-        *why = ps.why;
-        return -1;
-    }
     Nfa N;
-    Nfa::Frag f = N.build(ps.nodes, root);
+    Nfa::Frag f = N.build(nodes, root);
     int m = N.add(NState::MATCH);
     N.patch(f, m);
     if (N.too_big)
@@ -628,7 +621,7 @@ int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *w
     for (int c = 0; c < nc; c++) next[1][c] = 1;
     for (size_t s = 2; s < states.size(); s++)
     {
-        if (states.size() * (size_t)nc > budget_entries || states.size() > REGEX_MAX_STATES)
+        if (states.size() * (size_t)nc > budget_entries || states.size() > max_states)
         {
             *why = "the automaton has too many states";
             return -1;
@@ -688,34 +681,254 @@ int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *w
             else t = live[next[s][c]] ? next[s][c] : 1;
             D->trans[(size_t)s * nc + c] = (uint16_t)(t * nc); // entries are row offsets: next = trans[row + class]
         }
-    D->widened = ps.widened || N.widened;
+    D->widened = parse_widened || N.widened;
     D->count_exact = !D->widened;
     // offsets on the device: the plans whose per-line answer is exact, when the match automaton fits the shared memory
     // left next to the line table and the class map
     D->offsets_exact = false;
-    if (D->count_exact)
+    if (D->count_exact && smem_bytes)
     {
         const size_t used = (size_t)regex_tab_words((uint32_t)D->trans.size()) * 2 + 256;
-        const size_t budget = used < REGEX_SMEM_BYTES ? (REGEX_SMEM_BYTES - used) / 2 : 0;
+        // entries are 16-bit row offsets: a table of more than 65536 entries could not address its last rows
+        const size_t budget = std::min<size_t>(used < smem_bytes ? (smem_bytes - used) / 2 : 0, 65536);
         D->offsets_exact = build_match_automaton(N, start, cls, nc, rep, budget & ~(size_t)7, D);
         if (!D->offsets_exact) D->match.clear();
     }
     return 0;
 }
 
+// A split plan (DESIGN §12.7) of the top-level alternation `root`: its branches, in order, packed greedily into groups
+// of as many consecutive branches as one automaton holds (found by doubling the group, then bisecting), at most
+// REGEX_MAX_GROUPS of them, all in one image of REGEX_SET_SMEM_BYTES.  The packing compiles line automata only and
+// gives up as soon as the groups placed so far exceed the image or the group count; the match automata are built once,
+// for the final groups.  A group's match automaton may use what the image leaves; the sum over the groups decides
+// whether offsets stay on the device.
+int compile_split(std::vector<Ast> nodes, int root, bool parse_widened, uint32_t max_states, RegexDfa *D, std::string *why)
+{
+    const std::vector<int> br = nodes[root].kids;
+    auto compile_group = [&](size_t i, size_t k, RegexDfa *G, size_t smem_bytes) { // branches [i, i + k)
+        int r = br[i];
+        if (k > 1)
+        {
+            Ast a;
+            a.kind = Ast::ALT;
+            a.kids.assign(br.begin() + i, br.begin() + i + k);
+            nodes.push_back(a);
+            r = (int)nodes.size() - 1;
+        }
+        std::string w;
+        const bool ok = compile_automaton(nodes, r, parse_widened, max_states, smem_bytes, G, &w) == 0;
+        if (k > 1) nodes.pop_back();
+        return ok;
+    };
+    std::vector<RegexDfa> groups;
+    std::vector<std::pair<size_t, size_t>> spans; // the branches [first, first + count) of each group
+    size_t line_bytes = 0;
+    for (size_t i = 0; i < br.size();)
+    {
+        const size_t left = br.size() - i;
+        if (groups.size() == REGEX_MAX_GROUPS)
+        {
+            *why = "the alternation needs more automata than a split plan holds";
+            return -1;
+        }
+        RegexDfa best;
+        if (!compile_group(i, 1, &best, 0))
+        {
+            *why = "a branch of the alternation is too large for one automaton";
+            return -1;
+        }
+        size_t ok = 1, bad = i == 0 ? left : left + 1; // the whole alternation is known not to fit
+        for (size_t k = 2; k < bad; k *= 2)
+        {
+            RegexDfa g;
+            const size_t kk = std::min(k, left);
+            if (!compile_group(i, kk, &g, 0))
+            {
+                bad = kk;
+                break;
+            }
+            ok = kk;
+            best = std::move(g);
+            if (kk == left) break;
+        }
+        while (ok < left && bad - ok > 1)
+        {
+            RegexDfa g;
+            const size_t mid = ok + (bad - ok) / 2;
+            if (compile_group(i, mid, &g, 0)) ok = mid, best = std::move(g);
+            else bad = mid;
+        }
+        line_bytes += (size_t)regex_tab_words((uint32_t)best.trans.size()) * 2 + 256;
+        if (line_bytes > REGEX_SET_SMEM_BYTES)
+        {
+            *why = "the automata of the alternation exceed the shared memory of one scan";
+            return -1;
+        }
+        groups.push_back(std::move(best));
+        spans.push_back({i, ok});
+        i += ok;
+    }
+    bool widened = false;
+    for (const RegexDfa &g : groups) widened |= g.widened;
+    size_t match_bytes = 0;
+    bool matches = !widened;
+    for (size_t g = 0; g < groups.size() && matches; g++)
+    {
+        // the same line automaton again, now with its match automaton
+        matches = compile_group(spans[g].first, spans[g].second, &groups[g], REGEX_SET_SMEM_BYTES) && groups[g].offsets_exact;
+        match_bytes += (size_t)regex_tab_words((uint32_t)groups[g].match.size()) * 2;
+    }
+    D->widened = widened;
+    D->count_exact = !widened;
+    D->offsets_exact = D->count_exact && matches && line_bytes + match_bytes <= REGEX_SET_SMEM_BYTES;
+    if (!D->offsets_exact)
+        for (RegexDfa &g : groups) g.offsets_exact = false, g.match.clear();
+    D->groups = std::move(groups);
+    return 0;
+}
+
+} // namespace
+
+int regex_compile(const std::string &re, bool icase, RegexDfa *D, std::string *why, uint32_t max_states)
+{
+    if (MB_CUR_MAX != 1)
+    {
+        // krep never calls setlocale: its regexes are C-locale regexes.  A host running in a multibyte locale compiled
+        // a regex whose '.' and brackets match characters of several bytes, which a byte automaton does not model.
+        *why = "the process runs in a multibyte locale";
+        return -1;
+    }
+    Parser ps(re, icase);
+    int root = ps.parse_alt();
+    if (root >= 0 && ps.i != re.size()) root = ps.refuse("unmatched ')'");
+    if (root < 0)
+    {
+        *why = ps.why;
+        return -1;
+    }
+    // a regex one automaton holds is compiled as one; an alternation too large for one is split at its top level
+    if (compile_automaton(ps.nodes, root, ps.widened, max_states, REGEX_SMEM_BYTES, D, why) == 0) return 0;
+    if (ps.nodes[root].kind != Ast::ALT) return -1;
+    std::string whole = *why;
+    if (compile_split(std::move(ps.nodes), root, ps.widened, max_states, D, why) == 0) return 0;
+    *why = whole + "; " + *why;
+    return -1;
+}
+
+void regex_layout(const RegexDfa &D, RegexGroup *grp, uint32_t *ngroups, uint32_t *line_words, uint32_t *image_words)
+{
+    std::vector<const RegexDfa *> au;
+    if (D.groups.empty()) au.push_back(&D);
+    for (const RegexDfa &g : D.groups) au.push_back(&g);
+    uint32_t w = 0;
+    for (size_t g = 0; g < au.size(); g++)
+    {
+        grp[g].trans = w;
+        w += regex_tab_words((uint32_t)au[g]->trans.size());
+        grp[g].cls = w;
+        w += 128;
+        grp[g].nclasses = au[g]->nclasses;
+        grp[g].nl_class = au[g]->nl_class;
+        grp[g].start = au[g]->start;
+        grp[g].match_bol = au[g]->match_bol;
+        grp[g].match_mid = au[g]->match_mid;
+    }
+    *line_words = w;
+    for (size_t g = 0; g < au.size(); g++)
+    {
+        grp[g].match = w;
+        w += regex_tab_words((uint32_t)au[g]->match.size());
+    }
+    *image_words = w;
+    *ngroups = (uint32_t)au.size();
+    for (size_t g = au.size(); g < REGEX_MAX_GROUPS; g++)
+    {
+        // spare slots of the kernel's automata: the first group's, started DEAD (in both tables)
+        grp[g] = grp[0];
+        grp[g].start = grp[0].nclasses;
+        grp[g].match_bol = grp[g].match_mid = 0;
+    }
+}
+
+std::vector<uint16_t> regex_image(const RegexDfa &D)
+{
+    RegexGroup grp[REGEX_MAX_GROUPS];
+    uint32_t ng, lw, iw;
+    regex_layout(D, grp, &ng, &lw, &iw);
+    std::vector<uint16_t> img(iw, 0);
+    for (uint32_t g = 0; g < ng; g++)
+    {
+        const RegexDfa &A = D.groups.empty() ? D : D.groups[g];
+        std::copy(A.trans.begin(), A.trans.end(), img.begin() + grp[g].trans);
+        memcpy(img.data() + grp[g].cls, A.cls, 256);
+        std::copy(A.match.begin(), A.match.end(), img.begin() + grp[g].match);
+    }
+    return img;
+}
+
+namespace {
+
+// The line walk of a plan on the host, over its one automaton or the automata of a split plan: the line is MATCHED as
+// soon as one automaton is, DEAD once all are.
+struct LineWalk
+{
+    std::vector<const RegexDfa *> au;
+    std::vector<uint32_t> r;
+    enum { MATCHED, DEAD, LIVE } state = LIVE;
+
+    explicit LineWalk(const RegexDfa &D)
+    {
+        if (D.groups.empty()) au.push_back(&D);
+        for (const RegexDfa &g : D.groups) au.push_back(&g);
+        r.resize(au.size());
+    }
+    void settle()
+    {
+        state = DEAD;
+        for (size_t g = 0; g < au.size(); g++)
+        {
+            if (r[g] == 0)
+            {
+                state = MATCHED;
+                return;
+            }
+            if (r[g] > au[g]->nclasses) state = LIVE;
+        }
+    }
+    void begin()
+    {
+        for (size_t g = 0; g < au.size(); g++) r[g] = au[g]->start;
+        settle();
+    }
+    void step(uint8_t b)
+    {
+        for (size_t g = 0; g < au.size(); g++) r[g] = au[g]->trans[r[g] + au[g]->cls[b]];
+        settle();
+    }
+    void end_of_line() // the '\n' column of every live automaton
+    {
+        for (size_t g = 0; g < au.size(); g++)
+            if (r[g] > au[g]->nclasses) r[g] = au[g]->trans[r[g] + au[g]->nl_class];
+        settle();
+    }
+};
+
+} // namespace
+
 // The line filter run on the host — what k_regex_lines computes, without the kernel's long-line bound.
 void regex_lines_host(const RegexDfa &D, const char *t, size_t n, std::vector<uint64_t> *out)
 {
     out->clear();
-    const uint32_t nc = D.nclasses, dead = nc;
+    LineWalk W(D);
     size_t p = 0;
     while (p < n)
     {
-        uint32_t row = D.start;
+        W.begin();
         size_t q = p;
-        for (; q < n && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
-        if (row > dead) row = D.trans[row + D.nl_class]; // end of line (or of the text)
-        if (row == 0) out->push_back(p);
+        for (; q < n && t[q] != '\n' && W.state == LineWalk::LIVE; q++) W.step((uint8_t)t[q]);
+        if (W.state == LineWalk::LIVE) W.end_of_line(); // end of line (or of the text)
+        if (W.state == LineWalk::MATCHED) out->push_back(p);
         const void *nl = q < n ? memchr(t + q, '\n', n - q) : nullptr;
         if (!nl) break;
         p = (size_t)((const char *)nl - t) + 1;
@@ -728,20 +941,20 @@ void regex_lines_host(const RegexDfa &D, const char *t, size_t n, std::vector<ui
 uint64_t regex_count_lines_host(const RegexDfa &D, const char *t, size_t n, uint64_t reach, std::vector<uint64_t> *uncertain)
 {
     uncertain->clear();
-    const uint32_t dead = D.nclasses;
+    LineWalk W(D);
     uint64_t counted = 0;
     size_t p = 0;
     while (p < n)
     {
         const size_t limit = reach < n - p ? p + (size_t)reach : n;
-        uint32_t row = D.start;
+        W.begin();
         size_t q = p;
-        for (; q < limit && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
-        if (row > dead && q < limit) row = D.trans[row + D.nl_class]; // the walk stopped at the line's '\n'
-        if (row <= dead)
+        for (; q < limit && t[q] != '\n' && W.state == LineWalk::LIVE; q++) W.step((uint8_t)t[q]);
+        if (W.state == LineWalk::LIVE && q < limit) W.end_of_line(); // the walk stopped at the line's '\n'
+        if (W.state != LineWalk::LIVE)
             while (q < limit && t[q] != '\n') q++;
         if (q >= limit || q + 1 == n) uncertain->push_back(p); // '\n' out of reach, or the text's last byte
-        else if (row == 0) counted++;
+        else if (W.state == LineWalk::MATCHED) counted++;
         const void *nl = q < n ? memchr(t + q, '\n', n - q) : nullptr;
         if (!nl) break;
         p = (size_t)((const char *)nl - t) + 1;
@@ -752,27 +965,27 @@ uint64_t regex_count_lines_host(const RegexDfa &D, const char *t, size_t n, uint
 // The match mode of k_regex_lines (scan_regex.cu): the line walk of the count mode, then for a line decided MATCHED the
 // reference's loop restated inside the line [p, q] (q = its '\n'): from cur, the leftmost start s with a match and its
 // longest end e, emitted; cur = e, or s + 1 after an empty match; until cur passes q.  '^' holds only at s == p, '$'
-// only at q.  A line whose enumeration runs over its step budget leaves an uncertain key behind the match keys it
-// already emitted (the host drops those).
+// only at q.  A split plan tries every automaton at s: the match starts at the first s where one accepts and ends at the
+// longest of their ends, with G times the budget of one automaton.  A line whose enumeration runs over its step budget
+// leaves an uncertain key behind the match keys it already emitted (the host drops those).
 void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t reach, std::vector<uint64_t> *keys)
 {
     keys->clear();
-    const uint32_t dead = D.nclasses, nl = D.nl_class;
-    const uint16_t *M = D.match.data();
+    LineWalk W(D);
     size_t p = 0;
     while (p < n)
     {
         const size_t limit = reach < n - p ? p + (size_t)reach : n;
-        uint32_t row = D.start;
+        W.begin();
         size_t q = p;
-        for (; q < limit && t[q] != '\n' && row > dead; q++) row = D.trans[row + D.cls[(uint8_t)t[q]]];
-        if (row > dead && q < limit) row = D.trans[row + nl];
-        if (row <= dead)
+        for (; q < limit && t[q] != '\n' && W.state == LineWalk::LIVE; q++) W.step((uint8_t)t[q]);
+        if (W.state == LineWalk::LIVE && q < limit) W.end_of_line();
+        if (W.state != LineWalk::LIVE)
             while (q < limit && t[q] != '\n') q++;
         if (q >= limit || q + 1 == n) keys->push_back((uint64_t)p << REGEX_MATCH_SHIFT);
-        else if (row == 0)
+        else if (W.state == LineWalk::MATCHED)
         {
-            const uint64_t budget = (uint64_t)REGEX_MATCH_STEPS_PER_BYTE * (q - p) + REGEX_MATCH_STEPS_BASE;
+            const uint64_t budget = W.au.size() * ((uint64_t)REGEX_MATCH_STEPS_PER_BYTE * (q - p) + REGEX_MATCH_STEPS_BASE);
             uint64_t steps = 0;
             size_t cur = p;
             while (cur <= q && steps <= budget)
@@ -781,14 +994,19 @@ void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t rea
                 bool found = false;
                 for (; s <= q && steps <= budget; s++)
                 {
-                    uint32_t r = s == p ? D.match_bol : D.match_mid;
-                    steps++;
-                    if (M[r + nl] & (s == q ? RX_ACC_EOL : RX_ACC)) found = true, e = s;
-                    for (size_t x = s; x < q && r != 0;)
+                    for (const RegexDfa *A : W.au)
                     {
-                        r = M[r + D.cls[(uint8_t)t[x++]]];
+                        const uint16_t *M = A->match.data();
+                        const uint32_t nl = A->nl_class;
+                        uint32_t r = s == p ? A->match_bol : A->match_mid;
                         steps++;
-                        if (M[r + nl] & (x == q ? RX_ACC_EOL : RX_ACC)) found = true, e = x;
+                        if (M[r + nl] & (s == q ? RX_ACC_EOL : RX_ACC)) found = true, e = std::max(e, s);
+                        for (size_t x = s; x < q && r != 0;)
+                        {
+                            r = M[r + A->cls[(uint8_t)t[x++]]];
+                            steps++;
+                            if (M[r + nl] & (x == q ? RX_ACC_EOL : RX_ACC)) found = true, e = std::max(e, x);
+                        }
                     }
                     if (found) break;
                 }

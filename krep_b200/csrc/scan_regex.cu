@@ -19,9 +19,12 @@
 //   * in match mode (offsets on the device) the same walk decides the lines, and each line decided MATCHED is walked
 //     again with the anchored match automaton to emit one key per match, in the reference's order (DESIGN §12.2);
 //   * in batch mode (krep_b200_regex_search_batch) the text is many texts packed with '\n' gaps, and each line belongs
-//     to its own text: gap lines are skipped, each text's last line is uncertain, -c counts per text (DESIGN §12.5).
+//     to its own text: gap lines are skipped, each text's last line is uncertain, -c counts per text (DESIGN §12.5);
+//   * a split plan (DESIGN §12.7) runs the instantiations G = 2, 4, 8: the same walk over G automata at once, each byte
+//     read once and fed to all of them; the line is MATCHED when one of them is, DEAD when all are.
 //
-// Work per byte: one class lookup and one transition lookup in shared memory.
+// Work per byte: one class lookup and one transition lookup in shared memory per automaton.
+#include <atomic>
 #include <cooperative_groups.h>
 #include "common.h"
 #include "engine.h"
@@ -33,6 +36,9 @@ namespace kb {
 namespace {
 
 constexpr int RX_THREADS = 256;
+// split plans: an image of up to REGEX_SET_SMEM_BYTES leaves one CTA per SM, so the CTA is large; 512 threads keep
+// the 8-automaton instantiations within 128 registers without spills (ptxas, DESIGN §12.7)
+constexpr int RX_SET_THREADS = 512;
 constexpr uint32_t RX_SEG = REGEX_SEG; // bytes of owned range per thread
 
 // The aligned 16 bytes around the last position read, in registers.
@@ -114,6 +120,44 @@ enum RxMode : int
     RX_MATCH = 2,  // offsets: one key per match of a line decided MATCHED, uncertain lines leave keys
 };
 
+// The rows of the G automata of a split plan in one line walk, and the line's state from them in the row convention of
+// one automaton whose DEAD row is 1: 0 = MATCHED (one automaton matched), 1 = DEAD (all are dead), 2 = live.
+template <int G>
+struct SetRows
+{
+    uint32_t r[G];
+
+    __device__ __forceinline__ uint32_t state(const RegexLaunch &a) const
+    {
+        bool matched = false, live = false;
+#pragma unroll
+        for (int g = 0; g < G; g++)
+        {
+            matched |= r[g] == 0;
+            live |= r[g] > a.grp[g].nclasses;
+        }
+        return matched ? 0u : live ? 2u : 1u;
+    }
+    __device__ __forceinline__ void begin(const RegexLaunch &a)
+    {
+#pragma unroll
+        for (int g = 0; g < G; g++) r[g] = a.grp[g].start;
+    }
+    // G independent lookups: a DEAD automaton steps to DEAD
+    __device__ __forceinline__ void step(const RegexLaunch &a, const uint16_t *img, uint32_t b)
+    {
+        const uint8_t *bytes = reinterpret_cast<const uint8_t *>(img);
+#pragma unroll
+        for (int g = 0; g < G; g++) r[g] = img[a.grp[g].trans + r[g] + bytes[a.grp[g].cls * 2 + b]];
+    }
+    // the '\n' column: 0 where the automaton accepts at the end of the line, DEAD elsewhere (and for a DEAD one)
+    __device__ __forceinline__ void end_of_line(const RegexLaunch &a, const uint16_t *img)
+    {
+#pragma unroll
+        for (int g = 0; g < G; g++) r[g] = img[a.grp[g].trans + r[g] + a.grp[g].nl_class];
+    }
+};
+
 // Batch count mode: adds the thread's lines of text t to that text's counter.
 template <int MODE>
 __device__ __forceinline__ void add_text_lines(const RegexLaunch &a, uint32_t t, uint32_t &counted)
@@ -138,20 +182,26 @@ __device__ __forceinline__ void add_text_lines(const RegexLaunch &a, uint32_t t,
 // only if it still lies in the segment); in count and match mode the uncertain line is the one holding its own text's
 // last byte (its '\n' is the text's final byte or the gap's first); and count mode adds its lines to one counter per
 // text, once when the thread leaves a text and once at the end.
-template <int MODE, bool BATCH>
-__global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constant__ RegexLaunch a)
+// G == 1: the plan's one automaton.  G = 2, 4, 8: a split plan (DESIGN §12.7), its a.ngroups automata in the
+// first slots of G, the spare ones started DEAD; the walk runs on SetRows, and in match mode every automaton is tried at
+// each start: the match starts at the first start where one accepts and ends at the longest of their ends, within
+// a.ngroups times the step budget of one automaton.  Launch bounds: the split instantiations ask for one CTA per SM,
+// which lets ptxas give them up to 128 registers (without it, it holds them near 40 and spills); 0 leaves G == 1 as it was.
+template <int MODE, bool BATCH, int G>
+__global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ? 0 : 1) k_regex_lines(const __grid_constant__ RegexLaunch a)
 {
     extern __shared__ uint4 s_raw[];
     uint16_t *s_tab = reinterpret_cast<uint16_t *>(s_raw);
     const uint32_t tab_words = (a.ntrans + 7) & ~7u; // the class map follows the table, 16-byte aligned
-    // match mode: the match table follows the class map
-    const uint32_t nvec = (tab_words * 2 + 256 + (MODE == RX_MATCH ? regex_tab_words(a.nmtrans) * 2 : 0u)) / 16;
+    // match mode: the match table follows the class map (split plans: the match tables follow all line tables)
+    const uint32_t nvec = G > 1 ? (MODE == RX_MATCH ? a.image_words : a.line_words) / 8
+                                : (tab_words * 2 + 256 + (MODE == RX_MATCH ? regex_tab_words(a.nmtrans) * 2 : 0u)) / 16;
     const uint4 *src = reinterpret_cast<const uint4 *>(a.trans);
     for (uint32_t i = threadIdx.x; i < nvec; i += blockDim.x) s_raw[i] = src[i];
     __syncthreads();
     const uint8_t *s_cls = reinterpret_cast<const uint8_t *>(s_tab + tab_words);
     const uint16_t *s_mtab = s_tab + tab_words + 128;
-    const uint32_t dead = a.nclasses, nl = a.nl_class;
+    const uint32_t dead = G > 1 ? 1u : a.nclasses, nl = a.nl_class;
 
     const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
     const uint64_t nseg = (own + RX_SEG - 1) / RX_SEG;
@@ -202,19 +252,45 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
                     }
                 }
             }
-            uint32_t row = a.start;
+            uint32_t row;
             uint64_t q = p;
-            while (row > dead && q < limit)
+            SetRows<G> R;
+            if constexpr (G == 1)
             {
-                const uint32_t b = W.at(q);
-                if (b == '\n') break;
-                row = s_tab[row + s_cls[b]];
-                q++;
+                row = a.start;
+                while (row > dead && q < limit)
+                {
+                    const uint32_t b = W.at(q);
+                    if (b == '\n') break;
+                    row = s_tab[row + s_cls[b]];
+                    q++;
+                }
+            }
+            else
+            {
+                R.begin(a);
+                row = R.state(a);
+                while (row > dead && q < limit)
+                {
+                    const uint32_t b = W.at(q);
+                    if (b == '\n') break;
+                    R.step(a, s_tab, b);
+                    row = R.state(a);
+                    q++;
+                }
             }
             bool flag;
             if constexpr (MODE != RX_FILTER)
             {
-                if (row > dead && q < limit) row = s_tab[row + nl]; // the walk stopped at the line's '\n'
+                if constexpr (G == 1)
+                {
+                    if (row > dead && q < limit) row = s_tab[row + nl]; // the walk stopped at the line's '\n'
+                }
+                else if (row > dead && q < limit)
+                {
+                    R.end_of_line(a, s_tab);
+                    row = R.state(a);
+                }
                 if (row <= dead) q = next_newline(W, q, limit);
                 if constexpr (BATCH) flag = q >= limit || a.global_offset + q + 1 >= t_end; // out of reach, or its text's last byte
                 else flag = q >= limit || (q + 1 == a.avail_len && a.next_byte < 0); // '\n' out of reach, or the text's last byte
@@ -223,10 +299,58 @@ __global__ void __launch_bounds__(RX_THREADS) k_regex_lines(const __grid_constan
             else
             {
                 if (row <= dead) flag = row == 0;                                           // MATCHED / DEAD
-                else if (q < limit || (q == a.avail_len && a.next_byte < 0)) flag = s_tab[row + nl] == 0; // end of the line
+                else if (q < limit || (q == a.avail_len && a.next_byte < 0)) // end of the line
+                {
+                    if constexpr (G == 1) flag = s_tab[row + nl] == 0;
+                    else
+                    {
+                        R.end_of_line(a, s_tab);
+                        flag = R.state(a) == 0;
+                    }
+                }
                 else flag = true;                                                        // line not seen to its end: unverified
             }
-            if constexpr (MODE == RX_MATCH)
+            if constexpr (MODE == RX_MATCH && G > 1)
+            {
+                if (!flag && row == 0)
+                {
+                    const uint32_t len = (uint32_t)(q - p);
+                    const uint32_t budget = a.ngroups * (REGEX_MATCH_STEPS_PER_BYTE * len + REGEX_MATCH_STEPS_BASE);
+                    const uint8_t *bytes = reinterpret_cast<const uint8_t *>(s_tab);
+                    uint32_t steps = 0, cur = 0;
+                    while (cur <= len && steps <= budget)
+                    {
+                        uint32_t s = cur, e = 0;
+                        bool found = false;
+                        for (; s <= len && steps <= budget; s++)
+                        {
+#pragma unroll
+                            for (int g = 0; g < G; g++)
+                            {
+                                if (g >= (int)a.ngroups) break;
+                                const uint16_t *M = s_tab + a.grp[g].match;
+                                const uint8_t *cls = bytes + a.grp[g].cls * 2;
+                                const uint32_t gnl = a.grp[g].nl_class;
+                                uint32_t r = s == 0 ? a.grp[g].match_bol : a.grp[g].match_mid;
+                                steps++;
+                                if (M[r + gnl] & (s == len ? RX_ACC_EOL : RX_ACC)) found = true, e = max(e, s);
+                                for (uint32_t x = s; x < len && r != 0;)
+                                {
+                                    r = M[r + cls[W.at(p + x++)]];
+                                    steps++;
+                                    if (M[r + gnl] & (x == len ? RX_ACC_EOL : RX_ACC)) found = true, e = max(e, x);
+                                }
+                            }
+                            if (found) break;
+                        }
+                        if (!found) break;
+                        emit_key(a, ((a.global_offset + p + s) << REGEX_MATCH_SHIFT) | ((uint64_t)(e - s) << LIT_TAG_BITS) | 1);
+                        cur = e == s ? s + 1 : e;
+                    }
+                    flag = steps > budget; // over budget: the whole line goes to regexec
+                }
+            }
+            else if constexpr (MODE == RX_MATCH)
             {
                 if (!flag && row == 0)
                 {
@@ -291,7 +415,7 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
     const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256 + (MODE == RX_MATCH ? (size_t)regex_tab_words(a.nmtrans) * 2 : 0);
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE, BATCH>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE, BATCH, 1>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
     {
         cudaGetLastError();
         per_sm = 1;
@@ -302,12 +426,73 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
     trace("regex%s%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", BATCH ? " batch" : "",
           MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", grid, RX_THREADS, per_sm, smem);
-    k_regex_lines<MODE, BATCH><<<grid, RX_THREADS, smem, s>>>(a);
+    k_regex_lines<MODE, BATCH, 1><<<grid, RX_THREADS, smem, s>>>(a);
     count_launch();
 }
 
-void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
+template <int MODE, bool BATCH, int G>
+static int launch_regex_sets_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
+    const size_t smem = (size_t)(MODE == RX_MATCH ? a.image_words : a.line_words) * 2;
+    // above the default 48 KiB a kernel must opt in, once per device (the attribute belongs to the current device)
+    static std::atomic<bool> opted_in[MAX_DEV];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV)
+    {
+        set_error(-2, "regex scan: no current CUDA device (%s)", cudaGetErrorString(cudaGetLastError()));
+        return -2;
+    }
+    if (!opted_in[dev].load())
+    {
+        if (cudaFuncSetAttribute(k_regex_lines<MODE, BATCH, G>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)REGEX_SET_SMEM_BYTES) != cudaSuccess)
+        {
+            set_error(-2, "regex scan of %d automata: device %d refused %u bytes of dynamic shared memory (%s)", G, dev,
+                      REGEX_SET_SMEM_BYTES, cudaGetErrorString(cudaGetLastError()));
+            return -2;
+        }
+        opted_in[dev].store(true);
+    }
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE, BATCH, G>, RX_SET_THREADS, smem) != cudaSuccess ||
+        per_sm < 1)
+    {
+        cudaGetLastError();
+        per_sm = 1;
+    }
+    const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
+    const uint64_t blocks_needed = (own + (uint64_t)RX_SEG * RX_SET_THREADS - 1) / ((uint64_t)RX_SEG * RX_SET_THREADS);
+    const uint64_t resident = (uint64_t)sm_count * per_sm;
+    const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
+    trace("regex sets%s%s: %u automata, %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", BATCH ? " batch" : "",
+          MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", a.ngroups, grid, RX_SET_THREADS, per_sm, smem);
+    k_regex_lines<MODE, BATCH, G><<<grid, RX_SET_THREADS, smem, s>>>(a);
+    count_launch();
+    return 0;
+}
+
+template <int MODE, bool BATCH>
+static int launch_regex_sets(const RegexLaunch &a, int sm_count, cudaStream_t s)
+{
+    if (a.ngroups <= 2) return launch_regex_sets_t<MODE, BATCH, 2>(a, sm_count, s);
+    if (a.ngroups <= 4) return launch_regex_sets_t<MODE, BATCH, 4>(a, sm_count, s);
+    return launch_regex_sets_t<MODE, BATCH, 8>(a, sm_count, s);
+}
+
+int launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
+{
+    if (a.ngroups > 1)
+    {
+        if (a.text_end)
+        {
+            if (a.text_lines) return launch_regex_sets<RX_COUNT, true>(a, sm_count, s);
+            if (a.matches) return launch_regex_sets<RX_MATCH, true>(a, sm_count, s);
+            return launch_regex_sets<RX_FILTER, true>(a, sm_count, s);
+        }
+        if (a.line_count) return launch_regex_sets<RX_COUNT, false>(a, sm_count, s);
+        if (a.matches) return launch_regex_sets<RX_MATCH, false>(a, sm_count, s);
+        return launch_regex_sets<RX_FILTER, false>(a, sm_count, s);
+    }
     if (a.text_end)
     {
         if (a.text_lines) launch_regex_t<RX_COUNT, true>(a, sm_count, s);
@@ -317,6 +502,7 @@ void launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
     else if (a.line_count) launch_regex_t<RX_COUNT, false>(a, sm_count, s);
     else if (a.matches) launch_regex_t<RX_MATCH, false>(a, sm_count, s);
     else launch_regex_t<RX_FILTER, false>(a, sm_count, s);
+    return 0;
 }
 
 } // namespace kb
