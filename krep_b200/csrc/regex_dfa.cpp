@@ -3,9 +3,10 @@
 // one line (the bytes between two '\n') and tells whether the regex can match somewhere in it.
 //
 // The automaton is a filter, not a matcher.  It may say "yes" for a line glibc would not match (its answer is
-// widened wherever modelling glibc exactly would take effort: \b \B \< \> become empty, -i turns every bracket
-// expression into its case closure), never "no" for a line glibc matches.  Positions, leftmost-longest choice, -w, -c
-// and -m all come from glibc's regexec on the caller's own regex_t, run on the flagged lines only (replay_regex).
+// widened wherever modelling glibc exactly would take effort: \b \B \< \> become empty; an -i bracket expression whose
+// parsed set is not closed under case still marks the plan widened, though its bytes are glibc's own), never "no" for a
+// line glibc matches.  Positions, leftmost-longest choice, -w, -c and -m all come from glibc's regexec on the caller's
+// own regex_t, run on the flagged lines only (replay_regex).
 // Anything the parser does not know is refused, and a refused pattern stays on the host's regex_search.
 //
 // Under REG_NEWLINE (krep always sets it) no match contains a '\n' as long as no character set of the pattern contains
@@ -16,6 +17,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <regex.h>
 #include <string>
 #include <vector>
 #include "common.h"
@@ -253,8 +255,31 @@ struct Parser
         return true;
     }
 
+    // glibc's set of the bracket expression src under -i.  POSIX leaves case-insensitive ranges to the implementation,
+    // and glibc's answer is not the case closure of the range ([A-z] holds no byte of [\]^_`, [a-|] holds all six), so
+    // glibc is asked itself: the bracket alone, compiled as krep compiles -i regexes, against every byte but the newline.
+    // false when glibc refuses the bracket.
+    static bool icase_bracket(const std::string &src, CharSet *cs)
+    {
+        regex_t rx;
+        if (regcomp(&rx, src.c_str(), REG_EXTENDED | REG_NEWLINE | REG_ICASE) != 0) return false;
+        cs->reset();
+        for (int b = 0; b < 256; b++)
+        {
+            if (b == '\n') continue;
+            const char c = (char)b;
+            regmatch_t m;
+            m.rm_so = 0;
+            m.rm_eo = 1; // REG_STARTEND: the one byte, NUL included
+            if (regexec(&rx, &c, 1, &m, REG_STARTEND) == 0) (*cs)[b] = true;
+        }
+        regfree(&rx);
+        return true;
+    }
+
     int parse_bracket()
     {
+        const size_t open = i - 1; // the '['
         CharSet cs;
         bool neg = false;
         if (i < s.size() && s[i] == '^') neg = true, i++;
@@ -294,7 +319,12 @@ struct Parser
             cs.flip();
             cs['\n'] = false; // REG_NEWLINE: a non-matching list never matches the newline
         }
-        return set_node(cs, true);
+        // under -i, set_node decides refusal and widening from the case closure of the parsed set, as for every other
+        // set; the bytes the automaton reads are glibc's
+        const int n = set_node(cs, true);
+        if (n >= 0 && icase && !icase_bracket(s.substr(open, i - open), &nodes[n].set))
+            return refuse("a bracket expression glibc refuses under -i");
+        return n;
     }
 };
 
