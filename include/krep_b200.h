@@ -479,6 +479,15 @@ int64_t krep_b200_regex_matches_host(const search_params_t *params, const char *
  * No search entry point calls it. */
 int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
                                        uint64_t *keys, uint64_t cap, uint64_t *device_lines);
+/* Test hook: krep_b200_regex_scan_shard_raw followed by the long-line pass of the search entry points (DESIGN §12.8):
+ * the uncertain keys of lines whose '\n' lies beyond the kernel's reach but within avail_len (not the text's last line,
+ * shorter than 2^30 bytes) are decided on the device as the kernel would with unbounded reach.  slice_bytes and
+ * ckpt_bytes set the slice and checkpoint sizes (0: the production 4096 / 256); the output does not depend on them.
+ * Under KREP_B200_NO_LONG_LINES=1 it returns what krep_b200_regex_scan_shard_raw returns.  Errors as that hook's, and
+ * -3 for sizes outside 1 <= ckpt_bytes <= slice_bytes <= 2^20 with at most 1024 checkpoints per slice. */
+int64_t krep_b200_regex_scan_shard_long_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
+                                            uint32_t slice_bytes, uint32_t ckpt_bytes, uint64_t *keys, uint64_t cap,
+                                            uint64_t *device_lines);
 /* Test hook: how many automata the -E plan of params has — G >= 2 for a split plan (see krep_b200_regex_search), 1 for
  * a plan of one automaton, -1 when the pattern is refused. */
 int krep_b200_regex_automata(const search_params_t *params);

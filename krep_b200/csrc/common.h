@@ -66,6 +66,12 @@ static constexpr uint32_t REGEX_TABLE_BYTES = 32768; // transition table budget:
 static constexpr uint32_t REGEX_MAX_STATES = 4096;
 static constexpr uint32_t REGEX_HALO = 4096; // a line may run this far past its thread's segment before it is flagged unverified
 static constexpr uint32_t REGEX_SEG = 256;   // bytes of owned range per thread of k_regex_lines
+// The long-line pass (scan_regex_long.cu, DESIGN §12.8): a line whose '\n' lies beyond the reach of k_regex_lines is cut
+// into slices of REGEX_LONG_SLICE bytes walked in parallel, each recording its rows every REGEX_LONG_CKPT bytes.
+static constexpr uint32_t REGEX_LONG_SLICE = 4096;
+static constexpr uint32_t REGEX_LONG_CKPT = 256;
+static constexpr uint64_t REGEX_LONG_MAX_LINE = 1ull << 30; // longer lines stay with glibc (replay_regex cuts runs there)
+static constexpr uint32_t REGEX_LONG_MAX_MATCH = 8192;      // a match this long does not fit the match key's length field
 
 // Match mode of k_regex_lines (offsets on the device, DESIGN §12.2): one key per match of a line the device decides, one
 // per line it leaves to regexec.  Ascending key order is the reference's emission order; a line's uncertain key sorts
@@ -280,12 +286,21 @@ static constexpr uint64_t LB_SAME_AS_PREV = ~0ull;     // no newline between the
 static constexpr uint64_t LB_SAME_AS_NEXT = ~0ull - 1; // no newline between this occurrence and the next one
 static constexpr uint64_t LB_OUTSIDE_SHARD = ~0ull - 2; // the line continues into a neighbouring shard
 
+// Slice and checkpoint sizes of the long-line pass (0: REGEX_LONG_SLICE / REGEX_LONG_CKPT).
+struct LongLineOpts
+{
+    uint32_t slice_bytes = 0, ckpt_bytes = 0;
+};
+
 // Launch one shard scan on `stream` of the device context; appends to that device's key list (no counter reset).
 // regex_lines (regex plans only): run k_regex_lines in count mode, adding the lines it decides MATCHED there.
 // regex_matches (offsets_exact regex plans, with want_positions): run it in match mode (match and uncertain-line keys).
 // regex_batch: the shard is (a chunk of) a packed batch of texts; regex_lines then has one counter per text.
+// long_lines (regex plans, not batches): after k_regex_lines, decide the lines longer than its reach on the device
+// (scan_regex_long.cu, DESIGN §12.8); nullptr leaves them uncertain.
 int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0,
-                unsigned long long *regex_lines = nullptr, bool regex_matches = false, const RegexBatchDev *regex_batch = nullptr);
+                unsigned long long *regex_lines = nullptr, bool regex_matches = false, const RegexBatchDev *regex_batch = nullptr,
+                const LongLineOpts *long_lines = nullptr);
 // literal kernels (scan_literal.cu)
 void launch_literal(const Plan *plan, const LitDevParams &p, int sm_count, cudaStream_t s);
 // multi kernels (scan_multi.cu)
@@ -307,6 +322,11 @@ void launch_ac(const Plan *plan, const AcDevTables *T, const AcLaunch &a, int sm
 void count_launch(int n = 1);
 // regex kernel (scan_regex.cu)
 int launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s); // 0, or -2 with the error set
+// long-line pass (scan_regex_long.cu): long_lines_begin before launch_regex (scratch + list snapshot), launch_long_lines
+// after it, both on the scan's stream; 0, or the error set
+int long_lines_begin(DevCtx &C, const RegexLaunch &a, const LongLineOpts &o, cudaStream_t s);
+int launch_long_lines(DevCtx &C, const RegexLaunch &a, const LongLineOpts &o, cudaStream_t s);
+const LongLineOpts *long_lines_default(); // production sizes, or nullptr when KREP_B200_NO_LONG_LINES is set (read per call)
 
 // semantics.cpp — reference control flow replayed over the sorted occurrence list
 struct Replay

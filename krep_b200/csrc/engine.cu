@@ -274,6 +274,7 @@ static void ctx_destroy(DevCtx &E)
     cudaFreeHost(E.h_line_out);
     cudaFreeHost(E.h_keys);
     regex_pack_free(E);
+    long_lines_free(E);
     for (int s = 0; s < SCAN_SLOTS; s++)
     {
         cudaFree(E.d_pack[s]);
@@ -579,7 +580,7 @@ Plan *plan_build(const search_params_t *P, int algo, bool only_matching)
 // shard scan
 // ---------------------------------------------------------------------------------------------
 int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot,
-                unsigned long long *regex_lines, bool regex_matches, const RegexBatchDev *regex_batch)
+                unsigned long long *regex_lines, bool regex_matches, const RegexBatchDev *regex_batch, const LongLineOpts *long_lines)
 {
     if (((uintptr_t)sh->d_text & 15) != 0)
     {
@@ -629,7 +630,12 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.text_lines = regex_batch ? regex_lines : nullptr;
         a.n_texts = regex_batch ? regex_batch->n_texts : 0u;
         regex_layout(*plan->rx, a.grp, &a.ngroups, &a.line_words, &a.image_words);
-        return launch_regex(a, E.sm_count, stream);
+        // the long-line pass works on the keys this scan appends; batches keep every long line uncertain
+        const bool long_pass = long_lines && !regex_batch && a.cap > 0;
+        if (long_pass && long_lines_begin(E, a, *long_lines, stream) != 0) return -2;
+        const int rc = launch_regex(a, E.sm_count, stream);
+        if (rc != 0 || !long_pass) return rc;
+        return launch_long_lines(E, a, *long_lines, stream);
     }
     if (plan->is_ac)
     {
@@ -1256,9 +1262,9 @@ int krep_b200_scan_shard(const krep_b200_plan_t *plan, const krep_b200_shard_t *
 // sorted on the device: *d_sorted (device, *cnt keys; short lists sorted by k_finish into d_pack, longer ones by the radix
 // sort, enqueued on the stream) and the count mode's line counter.  Unlike scan_end's retry, an overflow re-scan keeps the
 // mode and zeroes the line counter again, so the keys and the count are those of one complete scan.  The lists stay valid
-// until the next scan on the device.
+// until the next scan on the device.  long_lines: the long-line pass follows the scan (DESIGN §12.8).
 int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt_out,
-                        const uint64_t **d_sorted, uint64_t *device_lines)
+                        const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines)
 {
     for (int s = 0; s < SCAN_SLOTS; s++)
         if (E.pend[s].active)
@@ -1276,7 +1282,7 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
         CK(cudaStreamWaitEvent(st, E.ev_done[slot], 0));
         if (reset_counter(E, slot, st) != 0) return -2;
         if (d_lines) CK(cudaMemsetAsync(d_lines, 0, sizeof(unsigned long long), st));
-        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2);
+        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2, nullptr, long_lines);
         if (rc != 0) return rc;
         if (finish_scan(E, slot, 1, st) != 0) return -2;
         if (d_lines) CK(cudaMemcpyAsync(E.h_line_out, d_lines, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -1303,21 +1309,22 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
 
 extern "C" {
 
-// One k_regex_lines scan in the given mode, its keys sorted and read back.
-int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep_b200_shard_t *shard, int mode, uint64_t *keys,
-                                       uint64_t cap, uint64_t *device_lines)
+// One k_regex_lines scan in the given mode (followed by the long-line pass when long_lines is set), its keys sorted and
+// read back.
+static int64_t regex_scan_raw(const char *who, const krep_b200_plan_t *plan_, const krep_b200_shard_t *shard, int mode,
+                              const LongLineOpts *long_lines, uint64_t *keys, uint64_t cap, uint64_t *device_lines)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
     clear_error();
     const Plan *plan = reinterpret_cast<const Plan *>(plan_);
     if (!plan || !shard || (cap && !keys))
     {
-        set_error(-3, "krep_b200_regex_scan_shard_raw: null argument");
+        set_error(-3, "%s: null argument", who);
         return -3;
     }
     if (!plan->is_regex || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
     {
-        set_error(-3, "krep_b200_regex_scan_shard_raw: mode %d is not available for this plan", mode);
+        set_error(-3, "%s: mode %d is not available for this plan", who, mode);
         return -3;
     }
     DeviceGuard guard;
@@ -1326,7 +1333,7 @@ int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep
     DevCtx &E = *Cp;
     uint64_t cnt = 0;
     const uint64_t *d_sorted = nullptr;
-    const int rc = regex_scan_keys(E, plan, shard, mode, "krep_b200_regex_scan_shard_raw", &cnt, &d_sorted, device_lines);
+    const int rc = regex_scan_keys(E, plan, shard, mode, who, &cnt, &d_sorted, device_lines, long_lines);
     if (rc != 0) return rc;
     const uint64_t n = cnt < cap ? cnt : cap;
     if (cnt <= PACK_KEYS)
@@ -1339,6 +1346,30 @@ int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan_, const krep
         CK(cudaStreamSynchronize(E.scan_stream));
     }
     return (int64_t)cnt;
+}
+
+int64_t krep_b200_regex_scan_shard_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode, uint64_t *keys,
+                                       uint64_t cap, uint64_t *device_lines)
+{
+    return regex_scan_raw("krep_b200_regex_scan_shard_raw", plan, shard, mode, nullptr, keys, cap, device_lines);
+}
+
+int64_t krep_b200_regex_scan_shard_long_raw(const krep_b200_plan_t *plan, const krep_b200_shard_t *shard, int mode,
+                                            uint32_t slice_bytes, uint32_t ckpt_bytes, uint64_t *keys, uint64_t cap,
+                                            uint64_t *device_lines)
+{
+    const char *who = "krep_b200_regex_scan_shard_long_raw";
+    LongLineOpts o;
+    o.slice_bytes = slice_bytes ? slice_bytes : REGEX_LONG_SLICE;
+    o.ckpt_bytes = ckpt_bytes ? ckpt_bytes : REGEX_LONG_CKPT;
+    if (o.slice_bytes > (1u << 20) || o.ckpt_bytes > o.slice_bytes || (o.slice_bytes + o.ckpt_bytes - 1) / o.ckpt_bytes > 1024)
+    {
+        clear_error();
+        set_error(-3, "%s: slices of 1 .. 2^20 bytes with checkpoints every 1 .. slice bytes, at most 1024 per slice (got %u / %u)",
+                  who, slice_bytes, ckpt_bytes);
+        return -3;
+    }
+    return regex_scan_raw(who, plan, shard, mode, long_lines_default() ? &o : nullptr, keys, cap, device_lines);
 }
 
 int krep_b200_export_keys(const krep_b200_device_result_t *dev, void *d_dst, uint64_t max_keys, void *stream)

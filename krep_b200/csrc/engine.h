@@ -33,6 +33,7 @@ struct PendingScan
 };
 
 struct RegexPackBufs;
+struct LongBufs;
 
 struct DevCtx
 {
@@ -83,6 +84,7 @@ struct DevCtx
     uint8_t *d_rx_batch = nullptr; // the text table of a krep_b200_regex_search_batch call (RegexBatchDev)
     size_t rx_batch_cap = 0;
     RegexPackBufs *rx_pack = nullptr; // -E rows of resident shards (scan_regex_pack.cu)
+    LongBufs *rx_long = nullptr;      // scratch of the -E long-line pass (scan_regex_long.cu)
 };
 
 // scan_regex_pack.cu — the -E row of a resident shard (layout: RegexRowHeader, csrc/common.h)
@@ -91,15 +93,17 @@ struct RegexPackStats
     float scan_ms = 0.f, pack_ms = 0.f; // device time: the k_regex_lines scan with its sort, and the pack kernels
     uint64_t packed_bytes = 0;          // row bytes
 };
-// One k_regex_lines scan of the shard in `mode` with its keys sorted on the device (engine.cu).
+// One k_regex_lines scan of the shard in `mode` with its keys sorted on the device (engine.cu); long_lines: followed by
+// the long-line pass (nullptr: not).
 int regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt,
-                    const uint64_t **d_sorted, uint64_t *device_lines);
+                    const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines = nullptr);
 // Packs the row of the shard whose sorted keys (nkeys, in `mode`'s layout) are at d_keys into engine-owned device memory
 // on the device's scan stream, and synchronises: *d_row, *row_bytes.  The row stays valid until the next pack on the device.
 int regex_pack_row(DevCtx &E, const krep_b200_shard_t *sh, int mode, const uint64_t *d_keys, uint64_t nkeys,
                    uint64_t device_lines, const void **d_row, uint64_t *row_bytes, float *pack_ms);
 uint8_t *regex_pack_host_buffer(DevCtx &E, uint64_t bytes); // pinned host room for a row read-back (grown as needed)
 void regex_pack_free(DevCtx &E);
+void long_lines_free(DevCtx &E);
 
 struct ErrState
 {

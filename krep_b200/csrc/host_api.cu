@@ -363,6 +363,7 @@ struct RangeJob
     uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
     bool regex_matches = false; // -E offsets on the device: match keys and uncertain-line keys (REGEX_MATCH_SHIFT layout)
     const RegexBatch *batch = nullptr; // -E batch: the text is packed texts; regex_count then counts per text
+    const LongLineOpts *long_lines = nullptr; // -E, not a batch: the long-line pass after each chunk's scan (DESIGN §12.8)
     std::vector<uint64_t> text_lines;  // batch, fused -c: lines of each text decided MATCHED in this range
     // results
     int rc = 0;
@@ -434,7 +435,7 @@ static int stream_range(RangeJob &J)
             CKH(cudaEventRecord(a, E.scan_stream));
             int rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
                                    : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines,
-                                                 J.regex_matches, J.batch ? &batch_dev : nullptr);
+                                                 J.regex_matches, J.batch ? &batch_dev : nullptr, J.long_lines);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
             CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
@@ -567,6 +568,7 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.regex_count = count_lines && plan->is_regex;
         J.regex_matches = regex_matches;
         J.batch = batch;
+        J.long_lines = plan->is_regex && !batch ? long_lines_default() : nullptr;
     }
     trace("search: %zu bytes (%s host memory), %zu device(s), %zu range(s), chunk %zu MiB", n, pinned ? "pinned" : "pageable", D, R,
           chunk >> 20);
@@ -965,7 +967,7 @@ static int regex_export(const Plan *plan, const search_params_t *P, const krep_b
     uint64_t cnt = 0, lines = 0;
     const uint64_t *d_sorted = nullptr;
     CKH(cudaEventRecord(C->ev_ca, C->scan_stream));
-    int rc = regex_scan_keys(*C, plan, sh, mode, who, &cnt, &d_sorted, &lines);
+    int rc = regex_scan_keys(*C, plan, sh, mode, who, &cnt, &d_sorted, &lines, long_lines_default());
     if (rc != 0) return rc;
     CKH(cudaEventRecord(C->ev_cb, C->scan_stream));
     float pack_ms = 0.f, scan_ms = 0.f;

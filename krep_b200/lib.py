@@ -124,6 +124,9 @@ def load():
     L.krep_b200_regex_scan_shard_raw.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.POINTER(C.c_uint64), C.c_uint64,
                                                  C.POINTER(C.c_uint64)]
     L.krep_b200_regex_scan_shard_raw.restype = C.c_int64
+    L.krep_b200_regex_scan_shard_long_raw.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.c_uint32, C.c_uint32,
+                                                      C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64)]
+    L.krep_b200_regex_scan_shard_long_raw.restype = C.c_int64
     L.krep_b200_regex_automata.argtypes = [C.POINTER(SearchParams)]
     L.krep_b200_regex_automata.restype = C.c_int
     L.krep_b200_regex_plan_split.argtypes = [C.POINTER(SearchParams), C.c_uint32]
