@@ -330,8 +330,10 @@ float krep_b200_last_kernel_ms(void);
 uint64_t krep_b200_launch_count(void);
 void krep_b200_reset_launch_count(void);
 
-/* Fused -c (count_lines_mode) for single literals: the scan itself counts the lines that hold an occurrence
- * (krep.c:1331-1351 and the equivalent branches of the other literal kernels), so only this record leaves the GPU.
+/* Fused -c (count_lines_mode): the lines that hold an occurrence are counted on the device, so only this record leaves
+ * the GPU.  Single literals count in the scan itself (krep.c:1331-1351 and the equivalent branches of the other literal
+ * kernels); pattern sets (aho_corasick.c:390-403) count from their sorted occurrence keys, which stay on the device, and a
+ * shard whose occurrences overflow the occurrence list is counted in pieces instead of growing the list.
  * A shard that cuts lines still gives an exact total: records of shards in text order are folded with
  * krep_b200_combine_line_counts, which subtracts a line counted on both sides of a cut. */
 typedef struct
@@ -347,9 +349,11 @@ enum
    KREP_B200_LINES_LAST_PENDING = 4, /* no newline between its last occurrence and its end (the line goes on)         */
    KREP_B200_LINES_HAS_NL = 8        /* the shard holds a newline (computed for shards without an occurrence)         */
 };
-/* Plans created from params with count_lines_mode set; not for pattern sets, needles of 17..64 bytes taken by the
- * window kernels, patterns containing a newline or -w plans in tag mode (those need krep_b200_scan_shard +
- * krep_b200_collect): returns a negative error for them. */
+/* Plans created from params with count_lines_mode set, single literals and pattern sets; not for needles of 17..64 bytes
+ * taken by the window kernels, patterns containing a newline (a set with one such pattern) or -w plans in tag mode (those
+ * need krep_b200_scan_shard + krep_b200_collect): returns -3 for them.  A pattern set's call waits for its scan's
+ * occurrence count before it enqueues the count itself, and fails with -3 while both scan slots of the device are held
+ * by krep_b200_scan_shard_begin. */
 int krep_b200_count_lines_shard(const krep_b200_plan_t *plan, const search_params_t *params, const krep_b200_shard_t *shard,
                                 void *stream, krep_b200_line_count_t *out);
 uint64_t krep_b200_combine_line_counts(const krep_b200_line_count_t *recs, size_t n, size_t max_count);
@@ -368,7 +372,8 @@ uint64_t krep_b200_collect(const krep_b200_plan_t *plan, const search_params_t *
  * chunk loop and merge (krep.c:2851-3004) for text that already lives in HBM.  Shards on distinct devices are scanned
  * concurrently, the per-shard lists merged by key, and the policy replayed ONCE over the whole list, so overlap rules,
  * -m and the emission order are those of the reference's single-chunk run.  -c is answered by the fused line count
- * (single literals; line cuts between shards are resolved).
+ * (single literals and pattern sets without a newline in a pattern; line cuts between shards are resolved, shards on
+ * distinct devices are counted concurrently).
  *
  * Regex plans (-E): returns the count and positions krep_b200_regex_search(params, text, n, result) returns on the text
  * the shards hold — the same path (fused -c, offsets on the device, or the line filter + regexec), the same knobs

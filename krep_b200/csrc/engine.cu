@@ -272,6 +272,7 @@ static void ctx_destroy(DevCtx &E)
     cudaFree(E.d_line_recs);
     cudaFree(E.d_line_out);
     cudaFreeHost(E.h_line_out);
+    cudaFree(E.d_set_acc);
     cudaFreeHost(E.h_keys);
     regex_pack_free(E);
     long_lines_free(E);
@@ -779,14 +780,15 @@ __global__ void __launch_bounds__(FIN_THREADS) k_finish(unsigned long long *coun
 // k_finish of the scan whose kernels were just enqueued on `stream`, on the same stream: being short, it is cheaper to run
 // it between two scans than beside one (a CTA that needs registers on an SM the scan's persistent CTAs already fill only
 // gets there when they exit, so an overlapped finish serialises anyway and slows the scan's tail).
-int finish_scan(DevCtx &E, int slot, int want_sort, cudaStream_t stream)
+int finish_scan(DevCtx &E, int slot, int want_sort, cudaStream_t stream, bool keys_to_host)
 {
     k_finish<<<PACK_KEYS / FIN_KEYS, FIN_THREADS, 0, stream>>>(slot_counter(E, slot), E.d_list[slot], E.key_cap, E.d_pack[slot],
                                                                  (want_sort && E.d_list[slot]) ? 1 : 0);
     CK(cudaGetLastError());
     // count + (possibly) sorted keys to the host in one DMA of the whole packed row: 128 KiB over PCIe is ~5 us, cheaper than
     // having the sort's scattered 8-byte stores go through mapped memory
-    CK(cudaMemcpyAsync(E.h_pack[slot], E.d_pack[slot], (want_sort ? PACK_KEYS + 1 : 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+    const size_t words = want_sort && keys_to_host ? PACK_KEYS + 1 : 1;
+    CK(cudaMemcpyAsync(E.h_pack[slot], E.d_pack[slot], words * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
     CK(cudaEventRecord(E.ev_done[slot], stream));
     count_launch();
     E.counter_clean[slot] = true;

@@ -69,6 +69,7 @@ struct DevCtx
     uint64_t line_recs_cap = 0;
     uint64_t *d_line_out = nullptr, *h_line_out = nullptr; // shard records (lines, flags), 2 words each; h_ is mapped pinned
     uint64_t line_out_cap = 0;
+    unsigned long long *d_set_acc = nullptr; // pattern-set -c (scan_set_count.cu): k_set_lines' two accumulators
     // host-text entry points: device ring the caller's buffer streams through + pinned staging ring + key read-back
     uint8_t *d_ring = nullptr;
     size_t ring_slot_bytes = 0;
@@ -142,7 +143,8 @@ unsigned long long *slot_counter(DevCtx &C, int slot);
 int scan_begin(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int *slot);
 int scan_end(DevCtx &C, int slot, ScanOut *out);
 int scan_shard(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, ScanOut *out);
-int finish_scan(DevCtx &C, int slot, int want_sort, cudaStream_t stream); // k_finish: count + small-list sort + counter reset
+// k_finish: count + small-list sort + counter reset; keys_to_host = false brings back the count only
+int finish_scan(DevCtx &C, int slot, int want_sort, cudaStream_t stream, bool keys_to_host = true);
 int ensure_keys(DevCtx &C, uint64_t cap);
 int reset_counter(DevCtx &C, int slot, cudaStream_t stream);
 int sort_keys(DevCtx &C, int slot, uint64_t n, int end_bit, cudaStream_t stream, const uint64_t **sorted);
@@ -159,6 +161,14 @@ bool count_lines_eligible(const Plan *plan, const search_params_t *P, int algo);
 int ensure_line_out(DevCtx &C, uint64_t n);
 int launch_count_lines(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, cudaStream_t stream, uint64_t index);
 uint64_t combine_line_records(const uint64_t *recs, size_t n); // records in text order -> number of matching lines
+
+// scan_set_count.cu — fused -c for pattern sets (count_lines_eligible AC plans).  set_count_begin enqueues the shard's
+// scan into the occurrence list of `slot` with k_finish (count only to the host); set_count_end waits for that count and
+// enqueues the record into E.h_line_out / E.d_line_out at `index` (synchronous when the list overflowed).  Work on one
+// slot must be ended before the slot is begun again; the other slot may be begun in between.
+int set_count_slot(const DevCtx &C); // a slot that no krep_b200_scan_shard_begin holds
+int set_count_begin(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, cudaStream_t stream, int slot);
+int set_count_end(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, cudaStream_t stream, int slot, uint64_t index);
 
 // Merges ascending key lists into dst (room for the sum of counts); lists of literal keys from rank-ordered shards are
 // already globally ordered, lists of pattern-set keys (ordered by END offset but owned by START offset) are not.

@@ -398,10 +398,21 @@ static int stream_range(RangeJob &J)
     if (J.batch && upload_regex_batch(E, *J.batch, &batch_dev) != 0) return -2;
     reset_kernel_ms();
     const int slot = 0;
+    // pattern-set -c: chunk c's scan is begun in list slot c % 2 before chunk c - 1 is ended (its record computed), so
+    // the host's wait for c - 1's count overlaps chunk c's copy; a chunk's ring slot is free again once it is ended
+    const bool set_count = J.count_lines && plan->is_ac;
+    krep_b200_shard_t set_part[SCAN_SLOTS];
+    auto set_end = [&](size_t c) -> int {
+        const int s = (int)(c % SCAN_SLOTS);
+        const int rc = set_count_end(E, plan, &set_part[s], E.scan_stream, s, c);
+        if (rc != 0) return rc;
+        CKH(cudaEventRecord(E.ring_scanned[c % E.ring_slots], E.scan_stream));
+        return 0;
+    };
     for (int attempt = 0; attempt < 3; attempt++)
     {
         CKH(cudaStreamWaitEvent(E.scan_stream, E.ev_done[slot], 0));
-        if (reset_counter(E, slot, E.scan_stream) != 0) return -2;
+        if (!set_count && reset_counter(E, slot, E.scan_stream) != 0) return -2;
         if (d_regex_lines) CKH(cudaMemsetAsync(d_regex_lines, 0, n_lines * sizeof(unsigned long long), E.scan_stream)); // also on a re-stage
         for (size_t c = 0; c < nchunks; c++)
         {
@@ -433,12 +444,25 @@ static int stream_range(RangeJob &J)
             part.next_byte = off + src_len < n ? (int32_t)(uint8_t)J.text[off + src_len] : -1;
             cudaEvent_t a = pool_event(E, 2 * c), b = pool_event(E, 2 * c + 1);
             CKH(cudaEventRecord(a, E.scan_stream));
-            int rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
+            int rc;
+            if (set_count)
+            {
+                set_part[c % SCAN_SLOTS] = part;
+                rc = set_count_begin(E, plan, &part, E.scan_stream, (int)(c % SCAN_SLOTS));
+            }
+            else
+                rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
                                    : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines,
                                                  J.regex_matches, J.batch ? &batch_dev : nullptr, J.long_lines);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
-            CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
+            if (!set_count) CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
+            else if (c > 0 && (rc = set_end(c - 1)) != 0) return rc;
+        }
+        if (set_count)
+        {
+            const int rc = set_end(nchunks - 1);
+            if (rc != 0) return rc;
         }
         CKH(cudaGetLastError());
         if (!J.count_lines && finish_scan(E, slot, J.want_positions, E.scan_stream) != 0) return -2;
@@ -1619,8 +1643,8 @@ int krep_b200_count_lines_shard(const krep_b200_plan_t *plan_, const search_para
     }
     if (!count_lines_eligible(plan, P, plan->algo))
     {
-        set_error(-3, "krep_b200_count_lines_shard: this plan's -c result needs the occurrence list (pattern set, window kernel, "
-                      "newline in the pattern or tag-mode -w): use krep_b200_scan_shard + krep_b200_collect");
+        set_error(-3, "krep_b200_count_lines_shard: this plan's -c result needs the occurrence list (window kernel, newline in "
+                      "a pattern or tag-mode -w): use krep_b200_scan_shard + krep_b200_collect");
         return -3;
     }
     DeviceGuard guard;
@@ -1691,7 +1715,7 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan_, const search_par
         if (!count_lines_eligible(plan, P, plan->algo))
         {
             set_error(-3, "krep_b200_search_shards: -c over several shards is only available where the scan counts lines itself "
-                          "(single literals; see krep_b200_count_lines_shard)");
+                          "(single literals and pattern sets; see krep_b200_count_lines_shard)");
             return 0;
         }
         if (P->max_count == 0) return 0;
@@ -1701,11 +1725,29 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan_, const search_par
             cudaSetDevice(ctx[i]->device);
             if (ensure_line_out(*ctx[i], n_shards) != 0) return 0;
         }
+        // a pattern set's record needs its scan's count on the host first: each device ends its previous shard before it
+        // begins the next one, so shards on distinct devices are scanned concurrently
+        std::vector<int> pending(MAX_DEV, -1);
+        auto set_end = [&](int i) {
+            DevCtx &C = *ctx[i];
+            cudaSetDevice(C.device);
+            return set_count_end(C, plan, &shards[i], C.scan_stream, set_count_slot(C), (uint64_t)i);
+        };
         for (uint32_t i = 0; i < n_shards; i++)
         {
-            cudaSetDevice(ctx[i]->device);
-            if (launch_count_lines(*ctx[i], plan, &shards[i], ctx[i]->scan_stream, i) != 0) return 0;
+            DevCtx &C = *ctx[i];
+            if (plan->is_ac && pending[C.device] >= 0 && set_end(pending[C.device]) != 0) return 0;
+            cudaSetDevice(C.device);
+            if (plan->is_ac)
+            {
+                if (set_count_begin(C, plan, &shards[i], C.scan_stream, set_count_slot(C)) != 0) return 0;
+                pending[C.device] = (int)i;
+            }
+            else if (launch_count_lines(C, plan, &shards[i], C.scan_stream, i) != 0)
+                return 0;
         }
+        for (int d = 0; d < MAX_DEV; d++)
+            if (pending[d] >= 0 && set_end(pending[d]) != 0) return 0;
         for (uint32_t i = 0; i < n_shards; i++)
         {
             cudaSetDevice(ctx[i]->device);

@@ -28,22 +28,10 @@
 // 3 bytes after the start); the pattern contains no newline, so proxy and start are on the same line.
 #include <algorithm>
 #include "engine.h"
+#include "line_rec.cuh"
 #include "lit_filters.cuh"
 
 namespace kb {
-
-enum : uint32_t
-{
-    LR_HAS_HIT = 1,      // at least one owned occurrence
-    LR_FIRST_OPEN = 2,   // the first occurrence lies before the first newline of the range (its line began earlier)
-    LR_LAST_PENDING = 4, // no newline between the last occurrence and the end of the range (its line goes on)
-    LR_HAS_NL = 8        // the range holds a newline (only meaningful, and only computed, for ranges without a hit)
-};
-
-struct LineRec
-{
-    uint32_t lines, flags;
-};
 
 struct CountDev
 {
@@ -64,26 +52,6 @@ struct PartState
 };
 
 __device__ __noinline__ unsigned verify_exact_call(const LitDevParams &p, long long cand) { return verify_exact(p, cand); }
-
-// 4-bit mask of the bytes of w that equal '\n' (exact per byte)
-__device__ __forceinline__ uint32_t nl_nibble(uint32_t w)
-{
-    const uint32_t x = w ^ 0x0A0A0A0Au;
-    const uint32_t y = ~(((x & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | x | 0x7F7F7F7Fu); // 0x80 in every zero byte of x
-    return ((y >> 7) * 0x10204080u) >> 28;
-}
-__device__ __forceinline__ uint32_t nl_mask16(const uint4 &v)
-{
-    return nl_nibble(v.x) | (nl_nibble(v.y) << 4) | (nl_nibble(v.z) << 8) | (nl_nibble(v.w) << 12);
-}
-// bits of a 16-byte unit at byte position `unit` that lie inside [lo, hi)
-__device__ __forceinline__ uint32_t range_mask16(uint64_t unit, uint64_t lo, uint64_t hi)
-{
-    uint32_t m = 0xFFFFu;
-    if (unit < lo) m = lo - unit >= 16 ? 0u : (m & ~((1u << (uint32_t)(lo - unit)) - 1u));
-    if (unit + 16 > hi) m = hi <= unit ? 0u : (m & ((1u << (uint32_t)(hi - unit)) - 1u));
-    return m;
-}
 
 // Is there a newline in bytes [lo, hi)?  Warp-cooperative, 512 bytes per step, stops at the first one.
 __device__ __noinline__ bool scan_for_newline(const LitDevParams &p, uint64_t lo, uint64_t hi)
@@ -375,29 +343,6 @@ __global__ void __launch_bounds__(256, KREP_B200_COUNT_MINB) k_count_lines(const
     }
 }
 
-// (lines, flags) of range A followed by range B
-__host__ __device__ __forceinline__ void append_rec(uint64_t &lines, uint32_t &flags, uint64_t blines, uint32_t bflags)
-{
-    const bool ah = flags & LR_HAS_HIT, bh = bflags & LR_HAS_HIT;
-    if (!bh)
-    {
-        if (ah && (bflags & LR_HAS_NL)) flags &= ~(uint32_t)LR_LAST_PENDING;
-        flags |= bflags & LR_HAS_NL;
-        return;
-    }
-    if (!ah)
-    {
-        const bool had_nl = flags & LR_HAS_NL;
-        lines = blines;
-        flags = bflags | LR_HAS_NL * had_nl;
-        if (had_nl) flags &= ~(uint32_t)LR_FIRST_OPEN;
-        return;
-    }
-    lines += blines;
-    if ((flags & LR_LAST_PENDING) && (bflags & LR_FIRST_OPEN)) lines--; // one line, counted on both sides of the cut
-    flags = LR_HAS_HIT | LR_HAS_NL | (flags & LR_FIRST_OPEN) | (bflags & LR_LAST_PENDING);
-}
-
 // Folds the partition records, in order, into one shard record: each thread folds a contiguous slice, thread 0 folds the
 // 1024 partial results.
 __global__ void __launch_bounds__(1024) k_count_finish(const LineRec *recs, uint32_t n, uint64_t *d_out, uint64_t *h_out)
@@ -440,10 +385,18 @@ __global__ void __launch_bounds__(1024) k_count_finish(const LineRec *recs, uint
     } while (0)
 
 // Does the fused count give exactly what the emulated kernel's -c replay gives?  (See the header comment; the window
-// kernels' tail sub-search recounts a straddling line, tag-mode -w plans need the cursor walk, prefix plans are -o.)
+// kernels' tail sub-search recounts a straddling line, tag-mode -w plans need the cursor walk, prefix plans are -o.
+// Pattern sets: scan_set_count.cu, as long as no pattern holds a newline.)
 bool count_lines_eligible(const Plan *plan, const search_params_t *P, int algo)
 {
-    if (!P->count_lines_mode || plan->is_ac || plan->is_regex || plan->emit_len != plan->m || plan->whole_word == 2) return false;
+    if (!P->count_lines_mode || plan->is_regex || plan->whole_word == 2) return false;
+    if (plan->is_ac)
+    {
+        for (const std::string &s : plan->patterns)
+            if (s.find('\n') != std::string::npos) return false;
+        return true;
+    }
+    if (plan->emit_len != plan->m) return false;
     if (plan->pattern.find('\n') != std::string::npos) return false;
     return algo == KREP_B200_ALGO_BMH || algo == KREP_B200_ALGO_KMP || algo == KREP_B200_ALGO_MEMCHR ||
            algo == KREP_B200_ALGO_MEMCHR_SHORT || algo == KREP_B200_ALGO_SSE42;
@@ -467,7 +420,8 @@ int ensure_line_out(DevCtx &E, uint64_t n)
 }
 
 // Enqueues the fused count of one shard on `stream`; its record lands in E.h_line_out[2*index .. 2*index+1] (mapped pinned
-// memory: readable after the stream is synchronised) and E.d_line_out likewise.
+// memory: readable after the stream is synchronised) and E.d_line_out likewise.  A pattern set's count waits for its
+// scan's occurrence count on the host before it enqueues the rest (scan_set_count.cu).
 int launch_count_lines(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, cudaStream_t stream, uint64_t index)
 {
     if (((uintptr_t)sh->d_text & 15) != 0)
@@ -478,6 +432,12 @@ int launch_count_lines(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh,
     const PlanDev *pd = plan_on_device(plan, E);
     if (!pd) return -2;
     if (ensure_line_out(E, index + 1) != 0) return -2;
+    if (plan->is_ac)
+    {
+        const int slot = set_count_slot(E);
+        const int rc = set_count_begin(E, plan, sh, stream, slot);
+        return rc != 0 ? rc : set_count_end(E, plan, sh, stream, slot, index);
+    }
     CountDev D;
     memset(&D, 0, sizeof D);
     LitDevParams &p = D.p;
