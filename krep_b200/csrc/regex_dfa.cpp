@@ -996,8 +996,9 @@ uint64_t regex_count_lines_host(const RegexDfa &D, const char *t, size_t n, uint
 // reference's loop restated inside the line [p, q] (q = its '\n'): from cur, the leftmost start s with a match and its
 // longest end e, emitted; cur = e, or s + 1 after an empty match; until cur passes q.  '^' holds only at s == p, '$'
 // only at q.  A split plan tries every automaton at s: the match starts at the first s where one accepts and ends at the
-// longest of their ends, with G times the budget of one automaton.  A line whose enumeration runs over its step budget
-// leaves an uncertain key behind the match keys it already emitted (the host drops those).
+// longest of their ends, with G times the budget of one automaton.  A line whose enumeration runs over its step budget,
+// or finds a match of REGEX_LONG_MAX_MATCH bytes or more (only lines past the kernel's reach have one; the long-line
+// pass does the same), leaves an uncertain key behind the match keys it already emitted (the host drops those).
 void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t reach, std::vector<uint64_t> *keys)
 {
     keys->clear();
@@ -1018,6 +1019,7 @@ void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t rea
             const uint64_t budget = W.au.size() * ((uint64_t)REGEX_MATCH_STEPS_PER_BYTE * (q - p) + REGEX_MATCH_STEPS_BASE);
             uint64_t steps = 0;
             size_t cur = p;
+            bool flag = false;
             while (cur <= q && steps <= budget)
             {
                 size_t s = cur, e = 0;
@@ -1041,10 +1043,15 @@ void regex_matches_host(const RegexDfa &D, const char *t, size_t n, uint64_t rea
                     if (found) break;
                 }
                 if (!found) break;
+                if (e - s >= REGEX_LONG_MAX_MATCH)
+                {
+                    flag = true; // the match does not fit the key's length field: the line goes to regexec whole
+                    break;
+                }
                 keys->push_back(((uint64_t)s << REGEX_MATCH_SHIFT) | ((uint64_t)(e - s) << LIT_TAG_BITS) | 1);
                 cur = e == s ? s + 1 : e;
             }
-            if (steps > budget) keys->push_back((uint64_t)p << REGEX_MATCH_SHIFT);
+            if (flag || steps > budget) keys->push_back((uint64_t)p << REGEX_MATCH_SHIFT);
         }
         const void *nlp = q < n ? memchr(t + q, '\n', n - q) : nullptr;
         if (!nlp) break;

@@ -18,6 +18,8 @@ and decides it as the kernel would with unbounded reach:
 
 Every other line is as in regex_kernel_model.expect.
 """
+import collections
+
 import numpy as np
 
 import regex_kernel_model as km
@@ -25,6 +27,29 @@ import regex_kernel_model as km
 MAX_LINE = 1 << 30
 MAX_MATCH = 8192
 SLICE, CKPT = 4096, 256  # production sizes (csrc/common.h)
+REC_BYTES = 64 << 20     # slice records of one round (scan_regex_long.cu)
+
+Sizes = collections.namedtuple("Sizes", "nck pick_cap owner_cap round_slices rounds")
+
+
+def width(ngroups):
+    """G of the pass's instantiation for a plan of ngroups automata: 1, 2, 4 or 8."""
+    return 1 if ngroups <= 1 else 2 if ngroups <= 2 else 4 if ngroups <= 4 else 8
+
+
+def sizes(avail, own, ngroups, slice=SLICE, ckpt=CKPT):
+    """The pass's scratch sizing (sizes_of): checkpoints per slice record, work-list and slice-map capacities, slices
+    per round (records of (S/C + 1) x G rows of 2 bytes, at most REC_BYTES a round) and the rounds launched."""
+    nck = (slice + ckpt - 1) // ckpt + 1
+    pick_cap = own // (km.REGEX_HALO + 1) + 2
+    owner_cap = (avail + slice - 1) // slice + pick_cap
+    round_slices = min(owner_cap, REC_BYTES // (nck * width(ngroups) * 2))
+    return Sizes(nck, pick_cap, owner_cap, round_slices, -(-owner_cap // round_slices))
+
+
+def slices_needed(sh, slice=SLICE):
+    """Slices the pass hands out for shard sh: ceil((nl - p) / slice) per taken line."""
+    return sum(-(-(nl - p) // slice) for p, nl in taken_lines(sh))
 
 
 def taken_lines(sh):

@@ -48,6 +48,35 @@ def test_taken_lines_follow_the_contract():
     assert lm.taken_lines(km.Shard(buf, 2, 300, prev_byte=ord("q"))) == [(3, 9003)]
 
 
+def test_sizes_follow_the_design():
+    # DESIGN §12.8: one round for a 256 MiB chunk and its halo, 3 for a 10 GiB shard at G = 1, 22 at G = 8
+    chunk = 256 << 20
+    assert lm.sizes(chunk + km.REGEX_HALO, chunk, 1).rounds == 1
+    assert lm.sizes(10 << 30, 10 << 30, 1).rounds == 3
+    z = lm.sizes(10 << 30, 10 << 30, 8)
+    assert z.rounds == 22 and z.nck == 17 and z.round_slices == (64 << 20) // 272
+    assert [lm.sizes(10 << 30, 10 << 30, n).rounds for n in (2, 3, 5, 7)] == [6, 11, 22, 22]
+    # the per-round slice counts the GPU tests size their texts from: slice 1 / checkpoint 1, and 1024 / 1
+    big = 1 << 30
+    assert [lm.sizes(big, big, g, 1, 1).round_slices for g in (1, 2, 4, 8)] == [16777216, 8388608, 4194304, 2097152]
+    assert [lm.sizes(big, big, g, 1024, 1).round_slices for g in (1, 8)] == [32736, 4092]
+    # a checkpoint that does not divide the slice adds a short last one; the round never exceeds the slice map
+    assert lm.sizes(100, 100, 1, 7, 3).nck == 4 and lm.sizes(100, 100, 1, 7, 3).round_slices == 17
+    assert lm.sizes(0, 0, 1).rounds == 1 and lm.sizes(0, 0, 1).pick_cap == 2
+    assert lm.sizes(1 << 20, 1 << 20, 1).pick_cap == (1 << 20) // 4097 + 2
+
+
+def test_slices_needed():
+    R = km.REGEX_SEG + km.REGEX_HALO
+    # lines of k*S - 1, k*S and k*S + 1 bytes: k, k and k + 1 slices; a line the pass does not take adds none
+    for n, want in ((2 * R - 1, 2), (2 * R, 2), (2 * R + 1, 3)):
+        sh = km.Shard(b"a" * n + b"\nb\n", 0, km.REGEX_SEG)
+        assert lm.slices_needed(sh, R) == want, n
+    sh = km.Shard(b"a" * (R - 1) + b"\n" + b"b" * 5000 + b"\n" + b"c" * 6000 + b"\n", 0, km.REGEX_SEG + R)
+    assert lm.taken_lines(sh) == [(R, R + 5000)]
+    assert lm.slices_needed(sh, 1) == 5000 and lm.slices_needed(sh) == 2
+
+
 @pytest.mark.parametrize("icase", [False, True])
 def test_model_plus_reference_is_the_reference(icase):
     rng = random.Random(11 + icase)
@@ -99,6 +128,16 @@ def test_long_match_keeps_the_key():
     lk = 0
     assert e.must_flag == {lk}
     assert e.prefix_lines[lk] == [(0 << 16) | (1 << 3) | 1]
+
+
+def test_host_twin_leaves_long_matches_to_regexec():
+    # krep_b200_regex_matches_host with unbounded reach (the GPU tests' oracle for long texts): a match of 8192 bytes or
+    # more does not fit the key's 13-bit length field, so the line goes to regexec whole, as in the long-line pass
+    for pats, body in ((["b|a+"], lambda n: b"b" + b"a" * n + b"b"), (["^[^x]*kqk"], lambda n: b"kqk" + b"c" * n + b"kqk")):
+        P = _params(pats, False)
+        for n in (8185, 8186, 8191, 8192, 16663, 30919):
+            text = b"x\n" + body(n) + b"\nz" * 3 + b"\n"
+            assert km.HookLines(P, text, P).pos == ru.ref_regex_search(P, text)[1], (pats, n)
 
 
 def test_equals_kernel_model_within_reach():
