@@ -183,7 +183,9 @@ int krep_b200_search_batch(search_func_t entry, const search_params_t *params, c
  * its own -m budget, -w, -i, -c, -co, and the early returns (max_count == 0, no compiled_regex, the empty text), which
  * are answered on the host without a launch.  The texts are packed at 16-byte aligned offsets with '\n' gaps, so no line
  * crosses from one text into the next; every text still costs at least one regexec call on its last line on the -c and
- * offsets paths.  A pattern krep_b200_regex_search refuses fails the call with -3 and every count 0.  Returns 0, or a
+ * offsets paths.  Lines longer than the line kernel's reach are decided on the GPU by the long-line pass, as in
+ * krep_b200_regex_search, except each text's last line and lines cut by a chunk edge; KREP_B200_NO_LONG_LINES=1 leaves
+ * them to regexec.  A pattern krep_b200_regex_search refuses fails the call with -3 and every count 0.  Returns 0, or a
  * negative error. */
 int krep_b200_regex_search_batch(const search_params_t *params, const char *const *texts, const size_t *lens,
                                  size_t n_texts, uint64_t *counts, match_result_t *const *results);
@@ -516,6 +518,16 @@ int64_t krep_b200_regex_plan_host(const krep_b200_plan_t *plan, int mode, const 
 int64_t krep_b200_regex_search_batch_raw(const search_params_t *params, const char *const *texts, const size_t *lens,
                                          size_t n_texts, int mode, uint64_t *offsets, uint64_t *keys, uint64_t cap,
                                          uint64_t *text_lines);
+/* Test hook: krep_b200_regex_search_batch_raw followed, after each chunk's scan, by the long-line pass of
+ * krep_b200_regex_search_batch (DESIGN §12.8) in the batch rules: a line is taken when its '\n' lies beyond the
+ * kernel's reach but within the chunk's readable bytes, it is not its own text's last line, and it is shorter than 2^30
+ * bytes.  In mode 1 its count goes to its text's text_lines.  slice_bytes and ckpt_bytes as for
+ * krep_b200_regex_scan_shard_long_raw (0: the production 4096 / 256); the output does not depend on them.  Under
+ * KREP_B200_NO_LONG_LINES=1 it returns what krep_b200_regex_search_batch_raw returns.  Errors as that hook's, and -3 for
+ * the sizes krep_b200_regex_scan_shard_long_raw refuses. */
+int64_t krep_b200_regex_search_batch_long_raw(const search_params_t *params, const char *const *texts, const size_t *lens,
+                                              size_t n_texts, int mode, uint32_t slice_bytes, uint32_t ckpt_bytes,
+                                              uint64_t *offsets, uint64_t *keys, uint64_t cap, uint64_t *text_lines);
 
 /* The same replay without any host text: `bounds` holds two words per key — the global offset of the first byte of
  * the occurrence's line and of that line's newline (or the text length) — as krep_b200_scan_shard computes them on

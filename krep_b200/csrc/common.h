@@ -296,8 +296,8 @@ struct LongLineOpts
 // regex_lines (regex plans only): run k_regex_lines in count mode, adding the lines it decides MATCHED there.
 // regex_matches (offsets_exact regex plans, with want_positions): run it in match mode (match and uncertain-line keys).
 // regex_batch: the shard is (a chunk of) a packed batch of texts; regex_lines then has one counter per text.
-// long_lines (regex plans, not batches): after k_regex_lines, decide the lines longer than its reach on the device
-// (scan_regex_long.cu, DESIGN §12.8); nullptr leaves them uncertain.
+// long_lines (regex plans): after k_regex_lines, decide the lines longer than its reach on the device
+// (scan_regex_long.cu, DESIGN §12.8), batches included; nullptr leaves them uncertain.
 int launch_scan(DevCtx &C, const Plan *plan, const krep_b200_shard_t *sh, int want_positions, cudaStream_t stream, int slot = 0,
                 unsigned long long *regex_lines = nullptr, bool regex_matches = false, const RegexBatchDev *regex_batch = nullptr,
                 const LongLineOpts *long_lines = nullptr);
@@ -327,6 +327,9 @@ int launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s); // 0, or -
 int long_lines_begin(DevCtx &C, const RegexLaunch &a, const LongLineOpts &o, cudaStream_t s);
 int launch_long_lines(DevCtx &C, const RegexLaunch &a, const LongLineOpts &o, cudaStream_t s);
 const LongLineOpts *long_lines_default(); // production sizes, or nullptr when KREP_B200_NO_LONG_LINES is set (read per call)
+// the sizes of the long-line test hooks (0: production); 0, or -3 with the error set for sizes outside
+// 1 <= ckpt <= slice <= 2^20 with at most 1024 checkpoints per slice
+int long_lines_opts(const char *who, uint32_t slice_bytes, uint32_t ckpt_bytes, LongLineOpts *o);
 
 // semantics.cpp — reference control flow replayed over the sorted occurrence list
 struct Replay

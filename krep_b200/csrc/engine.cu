@@ -631,8 +631,8 @@ int launch_scan(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh, int wa
         a.text_lines = regex_batch ? regex_lines : nullptr;
         a.n_texts = regex_batch ? regex_batch->n_texts : 0u;
         regex_layout(*plan->rx, a.grp, &a.ngroups, &a.line_words, &a.image_words);
-        // the long-line pass works on the keys this scan appends; batches keep every long line uncertain
-        const bool long_pass = long_lines && !regex_batch && a.cap > 0;
+        // the long-line pass works on the keys this scan appends (a batch's in the batch rules of k_regex_lines)
+        const bool long_pass = long_lines && a.cap > 0;
         if (long_pass && long_lines_begin(E, a, *long_lines, stream) != 0) return -2;
         const int rc = launch_regex(a, E.sm_count, stream);
         if (rc != 0 || !long_pass) return rc;
@@ -1362,15 +1362,7 @@ int64_t krep_b200_regex_scan_shard_long_raw(const krep_b200_plan_t *plan, const 
 {
     const char *who = "krep_b200_regex_scan_shard_long_raw";
     LongLineOpts o;
-    o.slice_bytes = slice_bytes ? slice_bytes : REGEX_LONG_SLICE;
-    o.ckpt_bytes = ckpt_bytes ? ckpt_bytes : REGEX_LONG_CKPT;
-    if (o.slice_bytes > (1u << 20) || o.ckpt_bytes > o.slice_bytes || (o.slice_bytes + o.ckpt_bytes - 1) / o.ckpt_bytes > 1024)
-    {
-        clear_error();
-        set_error(-3, "%s: slices of 1 .. 2^20 bytes with checkpoints every 1 .. slice bytes, at most 1024 per slice (got %u / %u)",
-                  who, slice_bytes, ckpt_bytes);
-        return -3;
-    }
+    if (long_lines_opts(who, slice_bytes, ckpt_bytes, &o) != 0) return -3;
     return regex_scan_raw(who, plan, shard, mode, long_lines_default() ? &o : nullptr, keys, cap, device_lines);
 }
 

@@ -327,6 +327,7 @@ struct RegexBatch
 {
     std::vector<uint64_t> start, end;
     std::vector<uint32_t> seg;
+    const LongLineOpts *long_lines = nullptr; // the long-line pass after each chunk's scan (nullptr: none)
 };
 
 // Copies the table to the device (on its scan stream, behind the scans before it).
@@ -363,7 +364,7 @@ struct RangeJob
     uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
     bool regex_matches = false; // -E offsets on the device: match keys and uncertain-line keys (REGEX_MATCH_SHIFT layout)
     const RegexBatch *batch = nullptr; // -E batch: the text is packed texts; regex_count then counts per text
-    const LongLineOpts *long_lines = nullptr; // -E, not a batch: the long-line pass after each chunk's scan (DESIGN §12.8)
+    const LongLineOpts *long_lines = nullptr; // -E: the long-line pass after each chunk's scan (DESIGN §12.8)
     std::vector<uint64_t> text_lines;  // batch, fused -c: lines of each text decided MATCHED in this range
     // results
     int rc = 0;
@@ -592,7 +593,7 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.regex_count = count_lines && plan->is_regex;
         J.regex_matches = regex_matches;
         J.batch = batch;
-        J.long_lines = plan->is_regex && !batch ? long_lines_default() : nullptr;
+        J.long_lines = !plan->is_regex ? nullptr : batch ? batch->long_lines : long_lines_default();
     }
     trace("search: %zu bytes (%s host memory), %zu device(s), %zu range(s), chunk %zu MiB", n, pinned ? "pinned" : "pageable", D, R,
           chunk >> 20);
@@ -1200,9 +1201,10 @@ static double ms_since(std::chrono::steady_clock::time_point t0)
 // packed with '\n' gaps (at least one '\n' after each text, up to the next 16-byte boundary), so that no line and no
 // automaton walk crosses from one text into the next, and scanned by stage_and_scan as one text in the kernel's batch
 // mode.  *off (indexed by f): packed offsets; *hs: the sorted keys in packed coordinates and, in mode 1, the device line
-// count of each live text (indexed like `live`).
+// count of each live text (indexed like `live`).  long_lines: the long-line pass after each chunk's scan, in the batch
+// rules (DESIGN §12.8); nullptr leaves every line past the kernel's reach uncertain.
 static int regex_batch_scan(const Plan *plan, const char *const *texts, const size_t *lens, const std::vector<size_t> &live,
-                            int mode, const char *who, std::vector<uint64_t> *off, HostScan *hs)
+                            int mode, const LongLineOpts *long_lines, const char *who, std::vector<uint64_t> *off, HostScan *hs)
 {
     if (live.size() >= UINT32_MAX)
     {
@@ -1216,6 +1218,7 @@ static int regex_batch_scan(const Plan *plan, const char *const *texts, const si
     if (pack_texts(*Cp, texts, lens, live, 1, '\n', off, &total) != 0) return -2;
     // the text table; seg[g]: the first text that ends after g * REGEX_SEG
     RegexBatch B;
+    B.long_lines = long_lines;
     const size_t nl = live.size();
     B.start.resize(nl);
     B.end.resize(nl);
@@ -1275,7 +1278,7 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
         const int mode = regex_call_mode(P, plan);
         std::vector<uint64_t> off(nt, 0);
         HostScan hs;
-        const int rc = regex_batch_scan(plan, texts, lens, live, mode, "krep_b200_regex_search_batch", &off, &hs);
+        const int rc = regex_batch_scan(plan, texts, lens, live, mode, long_lines_default(), "krep_b200_regex_search_batch", &off, &hs);
         if (rc != 0) return rc;
         const auto t0 = std::chrono::steady_clock::now();
         // keys ascend in packed coordinates: one pass cuts them per text (nothing outside a text is kept)
@@ -1392,23 +1395,24 @@ void krep_b200_regex_batch_stats(double *pack_ms, double *resolve_ms)
     if (resolve_ms) *resolve_ms = t_rx_batch.resolve_ms;
 }
 
-// One batch scan in the given mode, its keys sorted and read back (DESIGN §12.5).
-int64_t krep_b200_regex_search_batch_raw(const search_params_t *P, const char *const *texts, const size_t *lens, size_t n_texts,
-                                         int mode, uint64_t *offsets, uint64_t *keys, uint64_t cap, uint64_t *text_lines)
+// One batch scan in the given mode, its keys sorted and read back (DESIGN §12.5), with or without the long-line pass.
+static int64_t regex_batch_raw(const char *who, const search_params_t *P, const char *const *texts, const size_t *lens,
+                               size_t n_texts, int mode, const LongLineOpts *long_lines, uint64_t *offsets, uint64_t *keys,
+                               uint64_t cap, uint64_t *text_lines)
 {
     warm_join();
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
     clear_error();
     if (!P || (n_texts && (!texts || !lens)) || (cap && !keys))
     {
-        set_error(-3, "krep_b200_regex_search_batch_raw: null argument");
+        set_error(-3, "%s: null argument", who);
         return -3;
     }
     std::string why;
     Plan *plan = cached_regex_plan(P, &why);
     if (!plan || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
     {
-        set_error(-3, "krep_b200_regex_search_batch_raw: mode %d is not available for this pattern", mode);
+        set_error(-3, "%s: mode %d is not available for this pattern", who, mode);
         return -3;
     }
     std::vector<size_t> live;
@@ -1422,7 +1426,7 @@ int64_t krep_b200_regex_search_batch_raw(const search_params_t *P, const char *c
     DeviceGuard guard;
     std::vector<uint64_t> off(n_texts, 0);
     HostScan hs;
-    const int rc = regex_batch_scan(plan, texts, lens, live, mode, "krep_b200_regex_search_batch_raw", &off, &hs);
+    const int rc = regex_batch_scan(plan, texts, lens, live, mode, long_lines, who, &off, &hs);
     if (rc != 0) return rc;
     for (size_t i = 0; i < live.size(); i++)
     {
@@ -1431,6 +1435,24 @@ int64_t krep_b200_regex_search_batch_raw(const search_params_t *P, const char *c
     }
     if (hs.nkeys && cap) memcpy(keys, hs.keys, std::min<uint64_t>(hs.nkeys, cap) * sizeof(uint64_t));
     return (int64_t)hs.nkeys;
+}
+
+int64_t krep_b200_regex_search_batch_raw(const search_params_t *P, const char *const *texts, const size_t *lens, size_t n_texts,
+                                         int mode, uint64_t *offsets, uint64_t *keys, uint64_t cap, uint64_t *text_lines)
+{
+    return regex_batch_raw("krep_b200_regex_search_batch_raw", P, texts, lens, n_texts, mode, nullptr, offsets, keys, cap,
+                           text_lines);
+}
+
+int64_t krep_b200_regex_search_batch_long_raw(const search_params_t *P, const char *const *texts, const size_t *lens,
+                                              size_t n_texts, int mode, uint32_t slice_bytes, uint32_t ckpt_bytes,
+                                              uint64_t *offsets, uint64_t *keys, uint64_t cap, uint64_t *text_lines)
+{
+    const char *who = "krep_b200_regex_search_batch_long_raw";
+    LongLineOpts o;
+    if (long_lines_opts(who, slice_bytes, ckpt_bytes, &o) != 0) return -3;
+    return regex_batch_raw(who, P, texts, lens, n_texts, mode, long_lines_default() ? &o : nullptr, offsets, keys, cap,
+                           text_lines);
 }
 
 // krep.c:1873-1914

@@ -20,6 +20,9 @@
 //           a time, within the same step budget; a line over budget or with a match of REGEX_LONG_MAX_MATCH bytes or
 //           more keeps its uncertain key.
 //
+// Batches (krep_b200_regex_search_batch): pick, ends and chain take BATCH instantiations that find a picked line's
+// text, leave its own text's last line alone and count on its text's counter, as k_regex_lines<MODE, true, G> does.
+//
 // Slices are processed in rounds of at most round_slices so that the records stay within REC_BYTES.  Every kernel
 // returns at once when there is nothing to do, so a scan without long lines pays a few empty launches.
 #include <atomic>
@@ -98,6 +101,7 @@ struct LongBufs
     uint64_t rec_words = 0;
     uint64_t *tmp = nullptr;
     uint32_t *mlist = nullptr;
+    uint32_t *pick_text = nullptr; // batches: the text of each picked line
 };
 
 namespace {
@@ -143,8 +147,12 @@ __global__ void k_long_begin(const unsigned long long *counter, LongCtl *ctl)
 }
 
 // One warp per key appended by this scan: the line goes to the work list when no '\n' lies in [p, limit) and limit is
-// below avail_len.  Nothing is picked when the list overflowed (the scan is redone with a longer list).
-__global__ void __launch_bounds__(LL_THREADS) k_long_pick(const __grid_constant__ RegexLaunch a, const LongArgs L)
+// below avail_len.  Nothing is picked when the list overflowed (the scan is redone with a longer list).  BATCH: the
+// picked line's text goes to pick_text[idx], found as k_regex_lines finds it (its keys are never lines in a gap).
+// pick_text stays outside LongPick so that the single-text kernels keep their layout.
+template <bool BATCH>
+__global__ void __launch_bounds__(LL_THREADS) k_long_pick(const __grid_constant__ RegexLaunch a, const LongArgs L,
+                                                          uint32_t *pick_text)
 {
     const uint64_t snap = L.ctl->snap, end = a.counter[0];
     if (blockIdx.x == 0 && threadIdx.x == 0) L.ctl->end = end;
@@ -181,11 +189,22 @@ __global__ void __launch_bounds__(LL_THREADS) k_long_pick(const __grid_constant_
         P.key_idx = i;
         P.nslices = 0;
         P.state = PK_SKIP;
+        if constexpr (BATCH)
+        {
+            const uint64_t gp = a.global_offset + p;
+            uint32_t t = a.seg_text[gp / REGEX_SEG];
+            while (t + 1 < a.n_texts && a.text_end[t] <= gp) t++;
+            pick_text[idx] = t;
+        }
     }
 }
 
-// One CTA per picked line: its '\n' at or after limit (below p + REGEX_LONG_MAX_LINE and avail_len), its slices.
-__global__ void __launch_bounds__(LL_THREADS) k_long_ends(const __grid_constant__ RegexLaunch a, const LongArgs L)
+// One CTA per picked line: its '\n' at or after limit (below p + REGEX_LONG_MAX_LINE and avail_len), its slices.  The
+// line of the text's last byte is not taken: a single text's ('\n' at avail_len - 1, nothing after the shard), or in a
+// batch its own text's (the '\n' is the text's final byte or the gap's first: batch rule 2 of k_regex_lines).
+template <bool BATCH>
+__global__ void __launch_bounds__(LL_THREADS) k_long_ends(const __grid_constant__ RegexLaunch a, const LongArgs L,
+                                                          const uint32_t *pick_text)
 {
     __shared__ unsigned long long s_nl, s_base;
     __shared__ uint32_t s_ns;
@@ -219,7 +238,8 @@ __global__ void __launch_bounds__(LL_THREADS) k_long_ends(const __grid_constant_
             const uint64_t nl = s_nl;
             uint32_t ns = 0;
             s_base = 0;
-            if (nl != ~0ull && !(nl + 1 == a.avail_len && a.next_byte < 0))
+            if (nl != ~0ull && !(BATCH ? a.global_offset + nl + 1 >= a.text_end[pick_text[i]]
+                                       : nl + 1 == a.avail_len && a.next_byte < 0))
             {
                 ns = (uint32_t)((nl - p + L.slice - 1) / L.slice);
                 const unsigned long long base = atomicAdd(&L.ctl->nslices, (unsigned long long)ns);
@@ -303,9 +323,11 @@ __global__ void __launch_bounds__(G == 1 ? LL_THREADS : LL_SET_THREADS, G == 1 ?
     }
 }
 
-// The verdict of a line: the key goes (count, match), or goes unless MATCHED (filter); count mode counts it, match mode
-// queues it for k_long_match.
-__device__ __forceinline__ void decide(const RegexLaunch &a, const LongArgs &L, LongPick &P, uint32_t i, bool matched)
+// The verdict of a line: the key goes (count, match), or goes unless MATCHED (filter); count mode counts it (BATCH: on
+// its text's counter), match mode queues it for k_long_match.
+template <bool BATCH>
+__device__ __forceinline__ void decide(const RegexLaunch &a, const LongArgs &L, LongPick &P, uint32_t i, bool matched,
+                                       const uint32_t *pick_text)
 {
     if (L.mode == 0 && matched)
     {
@@ -316,14 +338,14 @@ __device__ __forceinline__ void decide(const RegexLaunch &a, const LongArgs &L, 
     P.state = PK_REMOVED;
     atomicAdd(&L.ctl->nremoved, 1ull);
     if (!matched) return;
-    if (L.mode == 1) atomicAdd(a.line_count, 1ull);
+    if (L.mode == 1) atomicAdd(BATCH ? a.text_lines + pick_text[i] : a.line_count, 1ull);
     else if (L.mode == 2) L.mlist[atomicAdd(&L.ctl->nmatch, 1ull)] = i;
 }
 
 // One thread per line with slices in this round: chains them in order (see the head of the file).
-template <int G>
+template <int G, bool BATCH>
 __global__ void __launch_bounds__(G == 1 ? LL_THREADS : LL_SET_THREADS, G == 1 ? 0 : 1)
-    k_long_chain(const __grid_constant__ RegexLaunch a, const LongArgs L, uint64_t r0)
+    k_long_chain(const __grid_constant__ RegexLaunch a, const LongArgs L, uint64_t r0, const uint32_t *pick_text)
 {
     extern __shared__ uint4 s_raw[];
     const uint16_t *img = reinterpret_cast<const uint16_t *>(s_raw);
@@ -380,7 +402,7 @@ __global__ void __launch_bounds__(G == 1 ? LL_THREADS : LL_SET_THREADS, G == 1 ?
             T.end_of_line(a, img); // the '\n' column
             st = T.state(a);
         }
-        decide(a, L, P, (uint32_t)i, st == 0);
+        decide<BATCH>(a, L, P, (uint32_t)i, st == 0, pick_text);
     }
 }
 
@@ -568,7 +590,8 @@ Sizes sizes_of(const RegexLaunch &a, const LongLineOpts &o)
     z.nck = (z.slice + z.ckpt - 1) / z.ckpt + 1;
     const uint64_t own = a.own_end > a.own_begin ? a.own_end - a.own_begin : 0;
     // picked lines are disjoint and each runs more than REGEX_HALO bytes past its start; every line adds at most one
-    // partial slice
+    // partial slice.  Both hold for a chunk of a packed batch as well: its lines, gaps included, are still disjoint and
+    // within avail_len, whichever texts they belong to.
     z.pick_cap = own / (REGEX_HALO + 1) + 2;
     z.owner_cap = (a.avail_len + z.slice - 1) / z.slice + z.pick_cap;
     const uint64_t g = a.ngroups > 1 ? (a.ngroups <= 2 ? 2 : a.ngroups <= 4 ? 4 : 8) : 1;
@@ -605,7 +628,8 @@ LongArgs args_of(const LongBufs &B, const Sizes &z, const RegexLaunch &a)
     L.slice = z.slice;
     L.ckpt = z.ckpt;
     L.nck = z.nck;
-    L.mode = a.line_count ? 1u : a.matches ? 2u : 0u;
+    // the mode k_regex_lines ran in (launch_regex): a batch counts on text_lines, a single text on line_count
+    L.mode = a.line_count || a.text_lines ? 1u : a.matches ? 2u : 0u;
     return L;
 }
 
@@ -646,22 +670,42 @@ int opt_in(K kernel, size_t smem, std::atomic<bool> *done)
     return 0;
 }
 
-template <int G>
-int launch_walks(const RegexLaunch &a, const LongArgs &L, const Sizes &z, int sm_count, cudaStream_t s)
+template <int G, bool BATCH>
+int launch_walks(const RegexLaunch &a, const LongArgs &L, const Sizes &z, int sm_count, cudaStream_t s, const uint32_t *pick_text)
 {
     const int threads = G == 1 ? LL_THREADS : LL_SET_THREADS;
     const size_t line_smem = (size_t)a.line_words * 2;
     static std::atomic<bool> done_slices[MAX_DEV], done_chain[MAX_DEV];
-    if (opt_in(k_long_slices<G>, line_smem, done_slices) || opt_in(k_long_chain<G>, line_smem, done_chain)) return -2;
+    if (opt_in(k_long_slices<G>, line_smem, done_slices) || opt_in(k_long_chain<G, BATCH>, line_smem, done_chain)) return -2;
     const unsigned gs = grid_for(k_long_slices<G>, threads, line_smem, sm_count, z.round_slices, threads);
-    const unsigned gc = grid_for(k_long_chain<G>, threads, line_smem, sm_count, z.pick_cap, threads);
+    const unsigned gc = grid_for(k_long_chain<G, BATCH>, threads, line_smem, sm_count, z.pick_cap, threads);
     for (uint64_t r = 0; r < z.rounds; r++)
     {
         k_long_slices<G><<<gs, threads, line_smem, s>>>(a, L, r * z.round_slices);
-        k_long_chain<G><<<gc, threads, line_smem, s>>>(a, L, r * z.round_slices);
+        k_long_chain<G, BATCH><<<gc, threads, line_smem, s>>>(a, L, r * z.round_slices, pick_text);
         count_launch(2);
     }
     return 0;
+}
+
+template <bool BATCH>
+int launch_walks_g(const RegexLaunch &a, const LongArgs &L, const Sizes &z, int sm_count, cudaStream_t s, const uint32_t *pick_text)
+{
+    const uint32_t G = a.ngroups <= 1 ? 1 : a.ngroups <= 2 ? 2 : a.ngroups <= 4 ? 4 : 8;
+    return G == 1 ? launch_walks<1, BATCH>(a, L, z, sm_count, s, pick_text)
+           : G == 2 ? launch_walks<2, BATCH>(a, L, z, sm_count, s, pick_text)
+           : G == 4 ? launch_walks<4, BATCH>(a, L, z, sm_count, s, pick_text)
+                    : launch_walks<8, BATCH>(a, L, z, sm_count, s, pick_text);
+}
+
+// the work list of one scan: picks and their ends (BATCH: with each line's text)
+template <bool BATCH>
+void launch_picks(const RegexLaunch &a, const LongArgs &L, const Sizes &z, int sm_count, cudaStream_t s, uint32_t *pick_text)
+{
+    k_long_pick<BATCH><<<grid_for(k_long_pick<BATCH>, LL_THREADS, 0, sm_count, 1ull << 20, LL_THREADS / 32), LL_THREADS, 0, s>>>(
+        a, L, pick_text);
+    k_long_ends<BATCH><<<grid_for(k_long_ends<BATCH>, LL_THREADS, 0, sm_count, z.pick_cap, 1), LL_THREADS, 0, s>>>(a, L, pick_text);
+    count_launch(2);
 }
 
 template <int G>
@@ -685,6 +729,20 @@ const LongLineOpts *long_lines_default()
     return getenv("KREP_B200_NO_LONG_LINES") ? nullptr : &prod;
 }
 
+int long_lines_opts(const char *who, uint32_t slice_bytes, uint32_t ckpt_bytes, LongLineOpts *o)
+{
+    o->slice_bytes = slice_bytes ? slice_bytes : REGEX_LONG_SLICE;
+    o->ckpt_bytes = ckpt_bytes ? ckpt_bytes : REGEX_LONG_CKPT;
+    if (o->slice_bytes > (1u << 20) || o->ckpt_bytes > o->slice_bytes || (o->slice_bytes + o->ckpt_bytes - 1) / o->ckpt_bytes > 1024)
+    {
+        clear_error();
+        set_error(-3, "%s: slices of 1 .. 2^20 bytes with checkpoints every 1 .. slice bytes, at most 1024 per slice (got %u / %u)",
+                  who, slice_bytes, ckpt_bytes);
+        return -3;
+    }
+    return 0;
+}
+
 int long_lines_begin(DevCtx &E, const RegexLaunch &a, const LongLineOpts &o, cudaStream_t s)
 {
     if (!E.rx_long) E.rx_long = new LongBufs();
@@ -693,18 +751,21 @@ int long_lines_begin(DevCtx &E, const RegexLaunch &a, const LongLineOpts &o, cud
     if (!B.ctl) CKL(cudaMalloc(&B.ctl, sizeof(LongCtl)));
     if (z.pick_cap > B.pick_cap)
     {
-        // the work list, the compaction's keys and the match list have one entry per picked line
+        // the work list, the compaction's keys, the match list and the lines' texts have one entry per picked line
         CKL(cudaDeviceSynchronize());
         cudaFree(B.picks);
         cudaFree(B.tmp);
         cudaFree(B.mlist);
+        cudaFree(B.pick_text);
         B.picks = nullptr;
         B.tmp = nullptr;
         B.mlist = nullptr;
+        B.pick_text = nullptr;
         B.pick_cap = 0;
         CKL(cudaMalloc(&B.picks, z.pick_cap * sizeof(LongPick)));
         CKL(cudaMalloc(&B.tmp, z.pick_cap * sizeof(uint64_t)));
         CKL(cudaMalloc(&B.mlist, z.pick_cap * sizeof(uint32_t)));
+        CKL(cudaMalloc(&B.pick_text, z.pick_cap * sizeof(uint32_t)));
         B.pick_cap = z.pick_cap;
     }
     if (grow((void **)&B.owner, &B.owner_cap, z.owner_cap, sizeof(uint32_t))) return -2;
@@ -721,15 +782,14 @@ int launch_long_lines(DevCtx &E, const RegexLaunch &a, const LongLineOpts &o, cu
     const LongBufs &B = *E.rx_long;
     const Sizes z = sizes_of(a, o);
     const LongArgs L = args_of(B, z, a);
-    k_long_pick<<<grid_for(k_long_pick, LL_THREADS, 0, E.sm_count, 1ull << 20, LL_THREADS / 32), LL_THREADS, 0, s>>>(a, L);
-    k_long_ends<<<grid_for(k_long_ends, LL_THREADS, 0, E.sm_count, z.pick_cap, 1), LL_THREADS, 0, s>>>(a, L);
-    count_launch(2);
-    const uint32_t G = a.ngroups <= 1 ? 1 : a.ngroups <= 2 ? 2 : a.ngroups <= 4 ? 4 : 8;
-    int rc = G == 1 ? launch_walks<1>(a, L, z, E.sm_count, s)
-             : G == 2 ? launch_walks<2>(a, L, z, E.sm_count, s)
-             : G == 4 ? launch_walks<4>(a, L, z, E.sm_count, s)
-                      : launch_walks<8>(a, L, z, E.sm_count, s);
+    // a batch (DESIGN §12.5): each picked line's text decides its last-line rule and takes its count
+    const bool batch = a.text_end != nullptr;
+    if (batch) launch_picks<true>(a, L, z, E.sm_count, s, B.pick_text);
+    else launch_picks<false>(a, L, z, E.sm_count, s, nullptr);
+    int rc = batch ? launch_walks_g<true>(a, L, z, E.sm_count, s, B.pick_text)
+                   : launch_walks_g<false>(a, L, z, E.sm_count, s, nullptr);
     if (rc != 0) return rc;
+    const uint32_t G = a.ngroups <= 1 ? 1 : a.ngroups <= 2 ? 2 : a.ngroups <= 4 ? 4 : 8;
     k_long_compact<<<1, 1024, 0, s>>>(a, L);
     count_launch();
     if (L.mode == 2)
@@ -741,8 +801,8 @@ int launch_long_lines(DevCtx &E, const RegexLaunch &a, const LongLineOpts &o, cu
         if (rc != 0) return rc;
     }
     CKL(cudaGetLastError());
-    trace("long lines: mode %u, slices of %u bytes, checkpoints every %u, %llu round(s)", L.mode, z.slice, z.ckpt,
-          (unsigned long long)z.rounds);
+    trace("long lines%s: mode %u, slices of %u bytes, checkpoints every %u, %llu round(s)", batch ? " (batch)" : "", L.mode,
+          z.slice, z.ckpt, (unsigned long long)z.rounds);
     return 0;
 }
 
@@ -756,6 +816,7 @@ void long_lines_free(DevCtx &E)
     cudaFree(B->rec);
     cudaFree(B->tmp);
     cudaFree(B->mlist);
+    cudaFree(B->pick_text);
     delete B;
     E.rx_long = nullptr;
 }

@@ -94,6 +94,10 @@ def load():
                                                    C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_uint64,
                                                    C.POINTER(C.c_uint64)]
     L.krep_b200_regex_search_batch_raw.restype = C.c_int64
+    L.krep_b200_regex_search_batch_long_raw.argtypes = [C.POINTER(SearchParams), C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                        C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64),
+                                                        C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64)]
+    L.krep_b200_regex_search_batch_long_raw.restype = C.c_int64
     L.krep_b200_scan_shard_begin.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.c_void_p, C.POINTER(C.c_int)]
     L.krep_b200_scan_shard_begin.restype = C.c_int
     L.krep_b200_scan_shard_end.argtypes = [C.c_int, C.POINTER(DeviceResult)]
