@@ -193,6 +193,35 @@ int krep_b200_regex_search_batch(const search_params_t *params, const char *cons
  * table) and the per-text replays.  The scan itself is krep_b200_last_kernel_ms. */
 void krep_b200_regex_batch_stats(double *pack_ms, double *resolve_ms);
 
+/* Many texts that already live in HBM, one call (DESIGN §12.9): text i is d_base[offsets[i] .. offsets[i] + lens[i]).
+ * d_base is device memory of one CUDA device, of any alignment (a torch tensor with a storage offset is fine); offsets
+ * and lens are host arrays; texts may come in any order, overlap or repeat.  counts[i] and results[i] are exactly what
+ * krep_b200_search_batch / krep_b200_regex_search_batch return for host copies of the same texts, with the same knobs.
+ * The texts are gathered on the device that owns d_base into one packed buffer (the host batch's layout), scanned there
+ * as one shard and resolved per text on the host from the keys (and, for -E, from one row of the lines glibc must
+ * see), so no text is copied to the host.  The packed buffer needs about the texts' total size in extra HBM; it is kept
+ * across calls and grown on demand, and a batch that cannot get it fails with -2.  Errors: -3 for a refused regex
+ * (every count 0), krep_b200_regex_search as entry (or any foreign entry), a d_base that is not device memory, or
+ * a span from the lowest text start to the highest text end that is not all mapped device memory; -2 for CUDA failures.
+ * The texts are read on the library's own stream: work that writes them on another stream must be complete before the
+ * call (synchronise that stream or the device).  Speed on an H100: README (bench_batch_resident.py). */
+int krep_b200_search_batch_resident(search_func_t entry, const search_params_t *params, const void *d_base,
+                                    const uint64_t *offsets, const size_t *lens, size_t n_texts, uint64_t *counts,
+                                    match_result_t *const *results);
+int krep_b200_regex_search_batch_resident(const search_params_t *params, const void *d_base, const uint64_t *offsets,
+                                          const size_t *lens, size_t n_texts, uint64_t *counts,
+                                          match_result_t *const *results);
+/* Times of the calling thread's most recent resident batch call: the gather kernel and the scan (with its sort and, for
+ * -E, the row pack) in device time, and the per-text replays on the host clock. */
+void krep_b200_batch_resident_stats(float *gather_ms, float *scan_ms, double *resolve_ms);
+/* Test hook: the packed buffer of a resident batch.  gap_kind 0: zero gaps of at least max_gap + 16 bytes (the literal
+ * and pattern-set batch, max_gap = the longest pattern); 1: '\n' gaps of at least one byte (the -E batch).  With base in
+ * device memory the texts are gathered by k_batch_gather; with base in host memory the host batch's own pack builds the
+ * buffer instead, for comparison.  Copies min(total, cap) bytes to dst_host and returns the total, or a negative error.
+ * No search entry point calls it. */
+int64_t krep_b200_batch_gather_raw(const void *base, const uint64_t *offsets, const size_t *lens, size_t n, int gap_kind,
+                                   size_t max_gap, void *dst_host, uint64_t cap);
+
 /* krep.c:1771 — same decision order, same globals.  For use_regex it returns
  * krep_b200_regex_search when the pattern's line automaton compiles, and
  * NULL when it is refused (the caller keeps its own regex_search then). */

@@ -6,7 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libkrep_b200.so")
-SOURCES = ["engine.cu", "scan_literal.cu", "scan_multi.cu", "scan_count.cu", "scan_set_count.cu", "scan_regex.cu", "scan_regex_long.cu", "scan_regex_pack.cu", "host_api.cu",
+SOURCES = ["engine.cu", "scan_literal.cu", "scan_multi.cu", "scan_count.cu", "scan_set_count.cu", "scan_regex.cu", "scan_regex_long.cu", "scan_regex_pack.cu", "scan_batch_gather.cu",
+           "host_api.cu",
            "semantics.cpp", "regex_dfa.cpp", "regex_rows.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

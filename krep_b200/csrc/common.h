@@ -373,6 +373,12 @@ uint64_t replay_regex_matches_windows(const search_params_t *P, const uint64_t *
 // regex_rows.cpp: the answer of a -E search from the rows of the shards that tile the text (text order).  *err: 0, or
 // -3 with the error set.
 uint64_t regex_resolve_rows(const search_params_t *P, const void *const *rows, uint32_t n_rows, match_result_t *res, int *err);
+// The answers of a packed -E batch from its one row (DESIGN §12.9).  Text i (packed order) is [lo[i], lo[i] + len[i]) of
+// the packed buffer, len[i] > 0, with last byte last[i] and, in count mode, text_lines[i] lines decided on the device;
+// counts[i] and res[i] (res or res[i] may be null) get krep_b200_regex_search's answer for it.  Returns 0, or -3 with
+// the error set.
+int regex_resolve_batch(const search_params_t *P, const void *row, size_t n_texts, const uint64_t *lo, const size_t *len,
+                        const uint8_t *last, const uint64_t *text_lines, uint64_t *counts, match_result_t *const *res);
 bool result_push(match_result_t *r, size_t s, size_t e);
 
 // C-locale helpers shared by host code (krep.c:125-134, krep.h:298-301)

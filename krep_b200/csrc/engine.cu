@@ -267,6 +267,8 @@ static void ctx_destroy(DevCtx &E)
     cudaFreeHost(E.h_bounds);
     cudaFreeHost(E.h_batch);
     cudaFree(E.d_rx_batch);
+    cudaFree(E.d_gather);
+    cudaFree(E.d_gather_tab);
     cudaFree(E.d_counter);
     cudaFree(E.d_ring);
     cudaFree(E.d_line_recs);
@@ -1266,7 +1268,7 @@ int krep_b200_scan_shard(const krep_b200_plan_t *plan, const krep_b200_shard_t *
 // mode and zeroes the line counter again, so the keys and the count are those of one complete scan.  The lists stay valid
 // until the next scan on the device.  long_lines: the long-line pass follows the scan (DESIGN §12.8).
 int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt_out,
-                        const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines)
+                        const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines, const RegexBatchDev *batch)
 {
     for (int s = 0; s < SCAN_SLOTS; s++)
         if (E.pend[s].active)
@@ -1274,7 +1276,8 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
             set_error(-3, "%s: a scan is in flight on device %d", who, E.device);
             return -3;
         }
-    if (ensure_keys(E, 1) != 0 || (mode == 1 && ensure_line_out(E, 1) != 0)) return -2;
+    const uint64_t n_lines = batch ? batch->n_texts : 1; // line counters: one per text of a batch
+    if (ensure_keys(E, 1) != 0 || (mode == 1 && ensure_line_out(E, (n_lines + 1) / 2) != 0)) return -2;
     unsigned long long *d_lines = mode == 1 ? (unsigned long long *)E.d_line_out : nullptr;
     const int slot = 0;
     cudaStream_t st = E.scan_stream;
@@ -1283,11 +1286,11 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
     {
         CK(cudaStreamWaitEvent(st, E.ev_done[slot], 0));
         if (reset_counter(E, slot, st) != 0) return -2;
-        if (d_lines) CK(cudaMemsetAsync(d_lines, 0, sizeof(unsigned long long), st));
-        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2, nullptr, long_lines);
+        if (d_lines) CK(cudaMemsetAsync(d_lines, 0, n_lines * sizeof(unsigned long long), st));
+        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2, batch, long_lines);
         if (rc != 0) return rc;
         if (finish_scan(E, slot, 1, st) != 0) return -2;
-        if (d_lines) CK(cudaMemcpyAsync(E.h_line_out, d_lines, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        if (d_lines) CK(cudaMemcpyAsync(E.h_line_out, d_lines, n_lines * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         const uint64_t cnt = E.h_pack[slot][0];
         if (cnt > E.key_cap)
@@ -1302,7 +1305,8 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
             if (rc != 0) return rc;
         }
         *cnt_out = cnt;
-        if (device_lines) *device_lines = d_lines ? E.h_line_out[0] : 0;
+        if (device_lines)
+            for (uint64_t i = 0; i < n_lines; i++) device_lines[i] = d_lines ? E.h_line_out[i] : 0;
         return 0;
     }
     set_error(-4, "occurrence list kept overflowing");

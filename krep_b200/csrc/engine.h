@@ -84,6 +84,12 @@ struct DevCtx
     uint64_t h_batch_cap = 0;
     uint8_t *d_rx_batch = nullptr; // the text table of a krep_b200_regex_search_batch call (RegexBatchDev)
     size_t rx_batch_cap = 0;
+    // resident batches (krep_b200_search_batch_resident, DESIGN §12.9): the packed texts, grown on demand and kept, and
+    // the gather table (source offset, packed offset, length per text) with one last byte per text after it
+    uint8_t *d_gather = nullptr;
+    uint64_t gather_cap = 0;
+    uint64_t *d_gather_tab = nullptr;
+    uint64_t gather_tab_cap = 0; // bytes
     RegexPackBufs *rx_pack = nullptr; // -E rows of resident shards (scan_regex_pack.cu)
     LongBufs *rx_long = nullptr;      // scratch of the -E long-line pass (scan_regex_long.cu)
 };
@@ -95,15 +101,22 @@ struct RegexPackStats
     uint64_t packed_bytes = 0;          // row bytes
 };
 // One k_regex_lines scan of the shard in `mode` with its keys sorted on the device (engine.cu); long_lines: followed by
-// the long-line pass (nullptr: not).
+// the long-line pass (nullptr: not).  batch: the shard is a packed -E batch with this text table, scanned in the
+// kernel's batch mode; the count mode then leaves one line count per text in device_lines[0 .. batch->n_texts).
 int regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt,
-                    const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines = nullptr);
+                    const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines = nullptr,
+                    const RegexBatchDev *batch = nullptr);
 // Packs the row of the shard whose sorted keys (nkeys, in `mode`'s layout) are at d_keys into engine-owned device memory
 // on the device's scan stream, and synchronises: *d_row, *row_bytes.  The row stays valid until the next pack on the device.
 int regex_pack_row(DevCtx &E, const krep_b200_shard_t *sh, int mode, const uint64_t *d_keys, uint64_t nkeys,
                    uint64_t device_lines, const void **d_row, uint64_t *row_bytes, float *pack_ms);
 uint8_t *regex_pack_host_buffer(DevCtx &E, uint64_t bytes); // pinned host room for a row read-back (grown as needed)
 void regex_pack_free(DevCtx &E);
+// scan_batch_gather.cu: k_batch_gather on stream st.  d_tab: nt source offsets (bytes from d_base), nt packed offsets
+// (ascending, 16-byte aligned), nt lengths; writes total bytes (a multiple of 16) to d_out, fill between the texts, and
+// each non-empty text's last byte to d_last[t] when d_last is set.
+int batch_gather(const void *d_base, const uint64_t *d_tab, uint32_t nt, uint64_t total, uint8_t fill, uint8_t *d_out,
+                 uint8_t *d_last, cudaStream_t st);
 void long_lines_free(DevCtx &E);
 
 struct ErrState

@@ -1068,10 +1068,10 @@ static uint64_t search_shards_regex(const Plan *plan, const search_params_t *P, 
     return err ? 0 : ret;
 }
 
-// Packs texts[f] for f in `live` (ascending) into the device's pinned batch buffer with the staging threads: text f at the
-// 16-byte aligned (*off)[f], followed by at least `gap` bytes of `fill` up to the next text's offset (or *total).
-static int pack_texts(DevCtx &E, const char *const *texts, const size_t *lens, const std::vector<size_t> &live, size_t gap,
-                      uint8_t fill, std::vector<uint64_t> *off, uint64_t *total)
+// The packed layout of a batch: text f (f in `live`, in that order) at the 16-byte aligned (*off)[f], followed by at
+// least `gap` bytes up to the next text's offset or the returned total.  The host pack (pack_texts) and the device
+// gather of resident batches (k_batch_gather) both place the texts by it.
+static uint64_t pack_layout(const size_t *lens, const std::vector<size_t> &live, size_t gap, std::vector<uint64_t> *off)
 {
     uint64_t t = 0;
     for (size_t f : live)
@@ -1079,6 +1079,15 @@ static int pack_texts(DevCtx &E, const char *const *texts, const size_t *lens, c
         (*off)[f] = t;
         t = (t + lens[f] + gap + 15) & ~15ull;
     }
+    return t;
+}
+
+// Packs texts[f] for f in `live` (ascending) into the device's pinned batch buffer with the staging threads, placed by
+// pack_layout, with `fill` in the gaps.
+static int pack_texts(DevCtx &E, const char *const *texts, const size_t *lens, const std::vector<size_t> &live, size_t gap,
+                      uint8_t fill, std::vector<uint64_t> *off, uint64_t *total)
+{
+    const uint64_t t = pack_layout(lens, live, gap, off);
     *total = t;
     if (t > E.h_batch_cap)
     {
@@ -1103,11 +1112,80 @@ static int pack_texts(DevCtx &E, const char *const *texts, const size_t *lens, c
     return 0;
 }
 
+// The early returns of a literal / pattern-set batch, text by text: counts[f] gets each early answer, algo_of[f] the
+// kernel of every other text.  text_of(f) stands for text f (only whether it is null is read).  Returns that kernel (the
+// resolved kernel depends on params only, except for the n < m early return), or -1 when every text was answered.
+template <class TextOf>
+static int batch_early_answers(int entry_algo, const search_params_t *P, size_t nt, const size_t *lens, TextOf text_of,
+                               uint64_t *counts, match_result_t *const *results, std::vector<int> *algo_of)
+{
+    algo_of->assign(nt, -1);
+    int algo = -1;
+    for (size_t f = 0; f < nt; f++)
+    {
+        int a = entry_algo;
+        uint64_t early = 0;
+        counts[f] = 0;
+        if (early_answer(entry_algo, P, text_of(f), lens[f], results ? results[f] : nullptr, &a, &early)) counts[f] = early;
+        else (*algo_of)[f] = algo = a;
+    }
+    return algo;
+}
+
+// Cuts the sorted key list of a packed literal / pattern-set batch per text — an occurrence belongs to a text only if
+// it lies wholly inside it — and replays each cut exactly as a separate call would have been (same early returns, own -m
+// limit, own line context), with Replay::base = the text's packed offset off[f].  texts: the host texts; nullptr
+// replays from the keys alone, as resident shards do, with -c taking `bounds` (two line bounds per key, in key order).
+static void replay_batch_cuts(const Plan *plan, int algo, const search_params_t *P, bool only_matching, const uint64_t *keys,
+                              uint64_t nkeys, const uint64_t *bounds, size_t gap, const std::vector<int> &algo_of,
+                              const std::vector<uint64_t> &off, const char *const *texts, const size_t *lens, uint64_t *counts,
+                              match_result_t *const *results)
+{
+    // texts are in ascending offset order; keys ascend by start, or by end for pattern sets
+    std::vector<uint64_t> mine, mine_bounds;
+    size_t j = 0;
+    for (size_t f = 0; f < algo_of.size(); f++)
+    {
+        if (algo_of[f] < 0) continue;
+        const uint64_t lo = off[f], hi = off[f] + lens[f];
+        mine.clear();
+        mine_bounds.clear();
+        while (j < nkeys)
+        {
+            uint64_t s, e;
+            if (plan->is_ac)
+            {
+                e = keys[j] >> AC_END_SHIFT;
+                s = e - (1024 - ((keys[j] >> AC_LEN_SHIFT) & 1023));
+            }
+            else
+            {
+                s = keys[j] >> LIT_TAG_BITS;
+                e = s + ((keys[j] >> 2) & 1 ? plan->m : plan->emit_len);
+            }
+            const uint64_t ord = plan->is_ac ? e : s; // the coordinate the list is sorted by
+            if (ord >= hi + (plan->is_ac ? gap : 0)) break; // belongs to a later text
+            if (s >= lo && e <= hi)
+            {
+                mine.push_back(keys[j]);
+                if (bounds)
+                {
+                    mine_bounds.push_back(bounds[2 * j]);
+                    mine_bounds.push_back(bounds[2 * j + 1]);
+                }
+            }
+            j++;
+        }
+        Replay r{mine.data(), mine.size(), texts ? texts[f] : nullptr, lens[f], lo, bounds ? mine_bounds.data() : nullptr};
+        match_result_t *res = results ? results[f] : nullptr;
+        counts[f] = plan->is_ac ? replay_ac(P, r, res) : replay_literal(algo, P, only_matching, plan->m, r, res);
+    }
+}
+
 // Many texts, one launch (SURVEY §8 f4: small files lose to launch and copy latency one by one).  The texts are packed
 // into one pinned buffer at 16-byte aligned offsets, separated by zero gaps longer than the longest pattern, copied and
-// scanned as ONE shard; the sorted occurrence list is then cut per text — an occurrence belongs to a text only if it
-// lies wholly inside it — and each cut is replayed exactly as a separate call would have been (same early returns, own
-// -m limit, own line context).  A gap byte is 0, i.e. not a word character: -w sees a text boundary there, as it should.
+// scanned as ONE shard; the sorted occurrence list is then cut per text and replayed (replay_batch_cuts).  A gap byte is
+// 0, i.e. not a word character: -w sees a text boundary there, as it should.
 static int run_batch(int entry_algo, const search_params_t *P, const char *const *texts, const size_t *lens, size_t nt,
                      uint64_t *counts, match_result_t *const *results)
 {
@@ -1120,16 +1198,8 @@ static int run_batch(int entry_algo, const search_params_t *P, const char *const
         return -3;
     }
     const bool only_matching = g_only_matching;
-    std::vector<int> algo_of(nt, -1);
-    int algo = -1;
-    for (size_t f = 0; f < nt; f++)
-    {
-        int a = entry_algo;
-        uint64_t early = 0;
-        counts[f] = 0;
-        if (early_answer(entry_algo, P, texts[f], lens[f], results ? results[f] : nullptr, &a, &early)) counts[f] = early;
-        else algo_of[f] = algo = a; // the resolved kernel depends on params only, except for the n < m early return above
-    }
+    std::vector<int> algo_of;
+    const int algo = batch_early_answers(entry_algo, P, nt, lens, [&](size_t f) { return texts[f]; }, counts, results, &algo_of);
     if (krep_b200_last_error() != 0) return -3;
     if (algo < 0) return 0; // every text was answered by an early return
     DeviceGuard guard;
@@ -1147,41 +1217,7 @@ static int run_batch(int entry_algo, const search_params_t *P, const char *const
     if (pack_texts(E, texts, lens, live, gap, 0, &off, &total) != 0) return -2;
     HostScan hs;
     if (stage_and_scan(plan, (const char *)E.h_batch, total, 1, &hs) != 0) return -2;
-    const uint64_t *keys = hs.keys;
-    struct { uint64_t stored; } so{hs.nkeys};
-    // cut the list per text (texts are in ascending offset order; keys ascend by start, or by end for pattern sets)
-    std::vector<uint64_t> mine;
-    size_t j = 0;
-    for (size_t f = 0; f < nt; f++)
-    {
-        if (algo_of[f] < 0) continue;
-        const uint64_t lo = off[f], hi = off[f] + lens[f];
-        mine.clear();
-        auto span = [&](uint64_t key, uint64_t *s, uint64_t *e) {
-            if (plan->is_ac)
-            {
-                *e = key >> AC_END_SHIFT;
-                *s = *e - (1024 - ((key >> AC_LEN_SHIFT) & 1023));
-            }
-            else
-            {
-                *s = key >> LIT_TAG_BITS;
-                *e = *s + ((key >> 2) & 1 ? plan->m : plan->emit_len);
-            }
-        };
-        while (j < so.stored)
-        {
-            uint64_t s, e;
-            span(keys[j], &s, &e);
-            const uint64_t ord = plan->is_ac ? e : s; // the coordinate the list is sorted by
-            if (ord >= hi + (plan->is_ac ? gap : 0)) break; // belongs to a later text
-            if (s >= lo && e <= hi) mine.push_back(keys[j]);
-            j++;
-        }
-        Replay r{mine.data(), mine.size(), texts[f], lens[f], lo};
-        match_result_t *res = results ? results[f] : nullptr;
-        counts[f] = plan->is_ac ? replay_ac(P, r, res) : replay_literal(algo, P, only_matching, plan->m, r, res);
-    }
+    replay_batch_cuts(plan, algo, P, only_matching, hs.keys, hs.nkeys, nullptr, gap, algo_of, off, texts, lens, counts, results);
     return 0;
 }
 
@@ -1195,6 +1231,27 @@ static thread_local RegexBatchTimes t_rx_batch; // of the most recent krep_b200_
 static double ms_since(std::chrono::steady_clock::time_point t0)
 {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
+// The text table of the texts f in `live` (ascending, lens[f] > 0) packed at off[f] into `total` bytes; seg[g]: the first
+// text that ends after g * REGEX_SEG.
+static void regex_batch_table(const size_t *lens, const std::vector<size_t> &live, const std::vector<uint64_t> &off, uint64_t total,
+                              RegexBatch *B)
+{
+    const size_t nl = live.size();
+    B->start.resize(nl);
+    B->end.resize(nl);
+    for (size_t i = 0; i < nl; i++)
+    {
+        B->start[i] = off[live[i]];
+        B->end[i] = B->start[i] + lens[live[i]];
+    }
+    B->seg.resize((total + REGEX_SEG - 1) / REGEX_SEG);
+    for (size_t g = 0, i = 0; g < B->seg.size(); g++)
+    {
+        while (i < nl && B->end[i] <= (uint64_t)g * REGEX_SEG) i++;
+        B->seg[g] = (uint32_t)i;
+    }
 }
 
 // One k_regex_lines scan in `mode` (0 filter, 1 fused -c, 2 offsets) of the texts f in `live` (ascending, lens[f] > 0):
@@ -1216,25 +1273,11 @@ static int regex_batch_scan(const Plan *plan, const char *const *texts, const si
     const auto t0 = std::chrono::steady_clock::now();
     uint64_t total = 0;
     if (pack_texts(*Cp, texts, lens, live, 1, '\n', off, &total) != 0) return -2;
-    // the text table; seg[g]: the first text that ends after g * REGEX_SEG
     RegexBatch B;
     B.long_lines = long_lines;
-    const size_t nl = live.size();
-    B.start.resize(nl);
-    B.end.resize(nl);
-    for (size_t i = 0; i < nl; i++)
-    {
-        B.start[i] = (*off)[live[i]];
-        B.end[i] = B.start[i] + lens[live[i]];
-    }
-    B.seg.resize((total + REGEX_SEG - 1) / REGEX_SEG);
-    for (size_t g = 0, i = 0; g < B.seg.size(); g++)
-    {
-        while (i < nl && B.end[i] <= (uint64_t)g * REGEX_SEG) i++;
-        B.seg[g] = (uint32_t)i;
-    }
+    regex_batch_table(lens, live, *off, total, &B);
     t_rx_batch.pack_ms += ms_since(t0);
-    trace("regex batch: %zu texts packed into %llu bytes", nl, (unsigned long long)total);
+    trace("regex batch: %zu texts packed into %llu bytes", live.size(), (unsigned long long)total);
     return stage_and_scan(plan, (const char *)Cp->h_batch, total, 1, hs, mode == 1, mode == 2, &B);
 }
 
@@ -1305,6 +1348,343 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
     return 0;
 }
 
+// ---- many HBM-resident texts in one call (DESIGN §12.9) ----
+struct ResidentTimes
+{
+    float gather_ms = 0.f, scan_ms = 0.f; // device time: k_batch_gather; the scan with its sort (and, -E, the row pack)
+    double resolve_ms = 0;                // host clock: the per-text replays
+};
+static thread_local ResidentTimes t_resident; // of the most recent resident batch call
+
+// The engine of the device that holds d_base, or nullptr with the error set: -3 when d_base is not device memory or
+// the bytes from the lowest text start to the highest text end are not all mapped device memory.  The check walks
+// the driver's cuMemGetAddressRange from the lowest start: a cudaMalloc allocation answers in one step, memory mapped
+// in several chunks (virtual memory management, such as torch's expandable segments) in one step per chunk, and an
+// unmapped hole refuses the call.  Without the driver entry point only d_base itself is checked.
+static DevCtx *resident_ctx(const char *who, const void *d_base, const uint64_t *offsets, const size_t *lens, size_t nt)
+{
+    cudaPointerAttributes a;
+    if (!d_base || cudaPointerGetAttributes(&a, d_base) != cudaSuccess || a.type != cudaMemoryTypeDevice)
+    {
+        cudaGetLastError();
+        set_error(-3, "%s: d_base is not device memory", who);
+        return nullptr;
+    }
+    uint64_t lo = UINT64_MAX, hi = 0;
+    for (size_t f = 0; f < nt; f++)
+        if (lens[f])
+        {
+            if (offsets[f] > UINT64_MAX - lens[f] || offsets[f] + lens[f] > UINT64_MAX - (uintptr_t)d_base)
+            {
+                set_error(-3, "%s: text %zu ends past the address space", who, f);
+                return nullptr;
+            }
+            lo = std::min<uint64_t>(lo, offsets[f]);
+            hi = std::max<uint64_t>(hi, offsets[f] + lens[f]);
+        }
+    if (hi > lo)
+    {
+        typedef int (*AddressRange)(unsigned long long *base, size_t *size, unsigned long long ptr);
+        static AddressRange range = [] {
+            void *fn = nullptr;
+            cudaDriverEntryPointQueryResult q;
+            if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
+            {
+                cudaGetLastError();
+                fn = nullptr;
+            }
+            return (AddressRange)fn;
+        }();
+        const unsigned long long end = (unsigned long long)(uintptr_t)d_base + hi;
+        unsigned long long p = (unsigned long long)(uintptr_t)d_base + lo;
+        while (range && p < end)
+        {
+            unsigned long long ab = 0;
+            size_t as = 0;
+            cudaPointerAttributes pa;
+            const bool mapped = range(&ab, &as, p) == 0 && as > 0 && ab + as > p &&
+                                cudaPointerGetAttributes(&pa, (const void *)(uintptr_t)p) == cudaSuccess &&
+                                pa.type == cudaMemoryTypeDevice && pa.device == a.device;
+            if (!mapped)
+            {
+                cudaGetLastError();
+                set_error(-3, "%s: the texts are not all in device memory of device %d (byte %llu from d_base is not)", who,
+                          a.device, (unsigned long long)(p - (uintptr_t)d_base));
+                return nullptr;
+            }
+            p = ab + as;
+        }
+    }
+    DevCtx *C = ctx_get(a.device);
+    if (C) cudaSetDevice(C->device);
+    return C;
+}
+
+// Packs the texts f in `live` (in that order) from d_base into E.d_gather on the device, placed by pack_layout with
+// `fill` in the gaps, as pack_texts packs host texts.  last: each text's last byte, indexed like live.
+static int gather_resident(DevCtx &E, const char *who, const void *d_base, const uint64_t *offsets, const size_t *lens,
+                           const std::vector<size_t> &live, size_t gap, uint8_t fill, std::vector<uint64_t> *off, uint64_t *total,
+                           std::vector<uint8_t> *last)
+{
+    *total = pack_layout(lens, live, gap, off);
+    const size_t nl = live.size();
+    if (*total > E.gather_cap)
+    {
+        CKH(cudaStreamSynchronize(E.scan_stream));
+        cudaFree(E.d_gather);
+        E.d_gather = nullptr;
+        E.gather_cap = 0;
+        const uint64_t want = *total + *total / 8 + 4096;
+        cudaError_t e = cudaMalloc(&E.d_gather, want);
+        if (e != cudaSuccess && (e = cudaMalloc(&E.d_gather, *total)) == cudaSuccess) E.gather_cap = *total;
+        else if (e == cudaSuccess) E.gather_cap = want;
+        if (e != cudaSuccess)
+        {
+            cudaGetLastError();
+            E.d_gather = nullptr;
+            set_error(-2, "%s: the packed batch needs %llu bytes of HBM on device %d, which cannot be allocated (%s); search the "
+                          "texts in smaller batches", who, (unsigned long long)*total, E.device, cudaGetErrorString(e));
+            return -2;
+        }
+    }
+    std::vector<uint64_t> tab(3 * nl);
+    for (size_t i = 0; i < nl; i++)
+    {
+        tab[i] = offsets[live[i]];
+        tab[nl + i] = (*off)[live[i]];
+        tab[2 * nl + i] = lens[live[i]];
+    }
+    const uint64_t tab_bytes = 24 * (uint64_t)nl + nl + 8;
+    if (tab_bytes > E.gather_tab_cap)
+    {
+        CKH(cudaStreamSynchronize(E.scan_stream));
+        cudaFree(E.d_gather_tab);
+        E.d_gather_tab = nullptr;
+        E.gather_tab_cap = 0;
+        CKH(cudaMalloc(&E.d_gather_tab, tab_bytes + tab_bytes / 4));
+        E.gather_tab_cap = tab_bytes + tab_bytes / 4;
+    }
+    cudaStream_t st = E.scan_stream;
+    uint8_t *d_last = last ? (uint8_t *)(E.d_gather_tab + 3 * nl) : nullptr;
+    if (nl) CKH(cudaMemcpyAsync(E.d_gather_tab, tab.data(), tab.size() * 8, cudaMemcpyHostToDevice, st));
+    cudaEvent_t a = pool_event(E, 0), b = pool_event(E, 1);
+    CKH(cudaEventRecord(a, st));
+    if (batch_gather(d_base, E.d_gather_tab, (uint32_t)nl, *total, fill, E.d_gather, d_last, st) != 0) return -2;
+    CKH(cudaEventRecord(b, st));
+    if (last)
+    {
+        last->resize(nl);
+        if (nl) CKH(cudaMemcpyAsync(last->data(), d_last, nl, cudaMemcpyDeviceToHost, st));
+    }
+    CKH(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    CKH(cudaEventElapsedTime(&ms, a, b));
+    t_resident.gather_ms += ms;
+    trace("%s: %zu texts gathered into %llu bytes (%.3f ms)", who, nl, (unsigned long long)*total, ms);
+    return 0;
+}
+
+// The packed buffer as one shard: it owns all its bytes and has no neighbours.
+static krep_b200_shard_t packed_shard(const DevCtx &E, uint64_t total)
+{
+    krep_b200_shard_t sh;
+    memset(&sh, 0, sizeof sh);
+    sh.d_text = E.d_gather;
+    sh.avail_len = total;
+    sh.own_begin = 0;
+    sh.own_end = total;
+    sh.global_offset = 0;
+    sh.prev_byte = -1;
+    sh.next_byte = -1;
+    return sh;
+}
+
+// krep_b200_search_batch_resident: krep_b200_search_batch's answers for texts that live in HBM.  The texts are gathered on
+// their device into one buffer laid out as run_batch packs host texts (gaps longer than the longest pattern), scanned as
+// one shard, and cut and replayed per text by replay_batch_cuts.  No host copy of a text exists, so each cut replays from
+// its keys alone, as resident shards do: -w from the tag bits the scan computed (a gap byte is not a word character, so a
+// text's edges read as text boundaries), and -c from the line bounds the scan of a count_lines plan found.  The gaps are
+// zero bytes, as on the host, except under -c, where they are '\n': the device's search for a line bound then stops at
+// the text's own edges, so it reads no byte of another text and finds the text's own find_line_start / find_line_end
+// (DESIGN §12.9).  No occurrence changes with the fill, since a key counts only when it lies wholly inside its text.
+static int run_batch_resident(int entry_algo, const search_params_t *P, const void *d_base, const uint64_t *offsets,
+                              const size_t *lens, size_t nt, uint64_t *counts, match_result_t *const *results)
+{
+    static const char *who = "krep_b200_search_batch_resident";
+    warm_join();
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    t_resident = ResidentTimes();
+    if (!P || (nt && (!offsets || !lens || !counts)))
+    {
+        set_error(-3, "%s: null argument", who);
+        return -3;
+    }
+    if (nt == 0) return 0;
+    for (size_t f = 0; f < nt; f++) counts[f] = 0;
+    if (visible_devices() == 0)
+    {
+        set_error(-1, "no CUDA device available; this engine has no CPU fallback");
+        return -1;
+    }
+    DeviceGuard guard;
+    DevCtx *Cp = resident_ctx(who, d_base, offsets, lens, nt);
+    if (!Cp) return krep_b200_last_error() ? krep_b200_last_error() : -1;
+    DevCtx &E = *Cp;
+    const bool only_matching = g_only_matching;
+    std::vector<int> algo_of;
+    const int algo = batch_early_answers(entry_algo, P, nt, lens, [&](size_t f) { return (const char *)d_base + offsets[f]; },
+                                         counts, results, &algo_of);
+    if (krep_b200_last_error() != 0) return -3;
+    if (algo < 0) return 0;
+    Plan *plan = plan_for(P, algo, only_matching);
+    if (!plan) return -2;
+    const size_t gap = (size_t)(plan->is_ac ? plan->max_len : plan->m) + 16;
+    std::vector<size_t> live;
+    for (size_t f = 0; f < nt; f++)
+        if (algo_of[f] >= 0) live.push_back(f);
+    if (live.size() >= UINT32_MAX)
+    {
+        set_error(-3, "%s: too many texts in one call", who);
+        return -3;
+    }
+    std::vector<uint64_t> off(nt, 0);
+    uint64_t total = 0;
+    const uint8_t fill = P->count_lines_mode ? '\n' : 0;
+    int rc = gather_resident(E, who, d_base, offsets, lens, live, gap, fill, &off, &total, nullptr);
+    if (rc != 0) return rc;
+    const krep_b200_shard_t sh = packed_shard(E, total);
+    ScanOut so;
+    if ((rc = scan_shard(E, plan, &sh, 1, E.scan_stream, &so)) != 0) return rc;
+    t_resident.scan_ms = get_kernel_ms();
+    const uint64_t *keys = nullptr;
+    if (fetch_keys(E, so, &keys) != 0) return -2;
+    // -c: the line bounds of every key, the "same line as my neighbour" markers resolved over the whole list (a '\n' gap
+    // lies between any two texts, so a marker never reaches into another text)
+    std::vector<uint64_t> bounds;
+    const bool lines = P->count_lines_mode && so.stored;
+    if (lines)
+    {
+        if (!so.d_bounds)
+        {
+            set_error(-2, "%s: the -c scan left no line bounds", who);
+            return -2;
+        }
+        bounds.resize(2 * so.stored);
+        CKH(cudaMemcpyAsync(bounds.data(), so.d_bounds, bounds.size() * 8, cudaMemcpyDeviceToHost, E.result_stream));
+        CKH(cudaStreamSynchronize(E.result_stream));
+        for (uint64_t i = 0; i < so.stored; i++)
+            if (bounds[2 * i] == LB_SAME_AS_PREV) bounds[2 * i] = i ? bounds[2 * (i - 1)] : 0;
+        for (uint64_t i = so.stored; i-- > 0;)
+            if (bounds[2 * i + 1] == LB_SAME_AS_NEXT) bounds[2 * i + 1] = i + 1 < so.stored ? bounds[2 * (i + 1) + 1] : total;
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    replay_batch_cuts(plan, algo, P, only_matching, keys, so.stored, lines ? bounds.data() : nullptr, gap, algo_of, off, nullptr,
+                      lens, counts, results);
+    t_resident.resolve_ms = ms_since(t0);
+    trace("%s: %zu texts, %llu keys (resolved in %.3f ms)", who, live.size(), (unsigned long long)so.stored, t_resident.resolve_ms);
+    return 0;
+}
+
+// krep_b200_regex_search_batch_resident: krep_b200_regex_search_batch's answers for texts that live in HBM.  The texts
+// are gathered on their device with '\n' gaps as regex_batch_scan packs host texts, scanned once in the kernel's batch
+// mode (with the long-line pass), and the bytes of the lines glibc must see come back in one row (scan_regex_pack.cu);
+// each text is then resolved from its part of the row (regex_resolve_batch) with its own length, last byte and -m
+// budget.  Empty texts keep the host answer.
+static int run_regex_batch_resident(const search_params_t *P, const void *d_base, const uint64_t *offsets, const size_t *lens,
+                                    size_t nt, uint64_t *counts, match_result_t *const *results)
+{
+    static const char *who = "krep_b200_regex_search_batch_resident";
+    warm_join();
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    t_resident = ResidentTimes();
+    if (!P || (nt && (!offsets || !lens || !counts)))
+    {
+        set_error(-3, "%s: null argument", who);
+        return -3;
+    }
+    if (nt == 0) return 0;
+    for (size_t f = 0; f < nt; f++) counts[f] = 0;
+    if (visible_devices() == 0)
+    {
+        set_error(-1, "no CUDA device available; this engine has no CPU fallback");
+        return -1;
+    }
+    DeviceGuard guard;
+    DevCtx *Cp = resident_ctx(who, d_base, offsets, lens, nt);
+    if (!Cp) return krep_b200_last_error() ? krep_b200_last_error() : -1;
+    DevCtx &E = *Cp;
+    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
+    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    std::vector<size_t> live;
+    for (size_t f = 0; f < nt; f++)
+        if (lens[f] > 0) live.push_back(f);
+    if (!live.empty())
+    {
+        std::string why;
+        Plan *plan = cached_regex_plan(P, &why);
+        if (!plan)
+        {
+            set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
+            return -3;
+        }
+        if (live.size() >= UINT32_MAX)
+        {
+            set_error(-3, "%s: too many texts in one call", who);
+            return -3;
+        }
+        const int mode = regex_call_mode(P, plan);
+        const size_t nl = live.size();
+        std::vector<uint64_t> off(nt, 0);
+        std::vector<uint8_t> last;
+        uint64_t total = 0;
+        int rc = gather_resident(E, who, d_base, offsets, lens, live, 1, '\n', &off, &total, &last);
+        if (rc != 0) return rc;
+        RegexBatch B;
+        regex_batch_table(lens, live, off, total, &B);
+        RegexBatchDev bd;
+        if (upload_regex_batch(E, B, &bd) != 0) return -2;
+        const krep_b200_shard_t sh = packed_shard(E, total);
+        uint64_t cnt = 0, row_bytes = 0;
+        const uint64_t *d_sorted = nullptr;
+        const void *d_row = nullptr;
+        std::vector<uint64_t> text_lines(nl, 0);
+        cudaEvent_t a = pool_event(E, 0), b = pool_event(E, 1);
+        CKH(cudaEventRecord(a, E.scan_stream));
+        if ((rc = regex_scan_keys(E, plan, &sh, mode, who, &cnt, &d_sorted, text_lines.data(), long_lines_default(), &bd)) != 0)
+            return rc;
+        CKH(cudaEventRecord(b, E.scan_stream));
+        float pack_ms = 0.f, scan_ms = 0.f;
+        if ((rc = regex_pack_row(E, &sh, mode, d_sorted, cnt, 0, &d_row, &row_bytes, &pack_ms)) != 0) return rc;
+        CKH(cudaEventElapsedTime(&scan_ms, a, b));
+        t_resident.scan_ms = scan_ms + pack_ms;
+        uint8_t *h = regex_pack_host_buffer(E, row_bytes);
+        if (!h) return -2;
+        CKH(cudaMemcpyAsync(h, d_row, row_bytes, cudaMemcpyDeviceToHost, E.scan_stream));
+        CKH(cudaStreamSynchronize(E.scan_stream));
+        const auto t0 = std::chrono::steady_clock::now();
+        std::vector<uint64_t> lo(nl), cnts(nl, 0);
+        std::vector<size_t> len(nl);
+        std::vector<match_result_t *> res(nl, nullptr);
+        for (size_t i = 0; i < nl; i++)
+        {
+            lo[i] = off[live[i]];
+            len[i] = lens[live[i]];
+            if (results) res[i] = results[live[i]];
+        }
+        if ((rc = regex_resolve_batch(P, h, nl, lo.data(), len.data(), last.data(), text_lines.data(), cnts.data(), res.data())) != 0)
+            return rc;
+        for (size_t i = 0; i < nl; i++) counts[live[i]] = cnts[i];
+        t_resident.resolve_ms = ms_since(t0);
+        trace("%s: mode %d, %zu texts, %llu keys, %llu row bytes (resolved in %.3f ms)", who, mode, nl, (unsigned long long)cnt,
+              (unsigned long long)row_bytes, t_resident.resolve_ms);
+    }
+    for (size_t f = 0; f < nt; f++)
+        if (lens[f] == 0) counts[f] = replay_regex(P, Replay{nullptr, 0, "", 0, 0}, results ? results[f] : nullptr); // krep.c:1403
+    return 0;
+}
+
 } // namespace kb
 
 using namespace kb;
@@ -1357,8 +1737,15 @@ uint64_t krep_b200_regex_search(const search_params_t *p, const char *t, size_t 
     return run_regex(p, t, n, r);
 }
 
-int krep_b200_search_batch(search_func_t entry, const search_params_t *params, const char *const *texts, const size_t *lens,
-                           size_t n_texts, uint64_t *counts, match_result_t *const *results)
+
+int krep_b200_regex_search_batch(const search_params_t *params, const char *const *texts, const size_t *lens, size_t n_texts,
+                                 uint64_t *counts, match_result_t *const *results)
+{
+    return run_regex_batch(params, texts, lens, n_texts, counts, results);
+}
+
+// The kernel a batch entry point emulates, or -1 with the error set (regex_batch: the call that batches regex searches).
+static int batch_entry_algo(search_func_t entry, const char *who, const char *regex_batch)
 {
     int algo = -1;
     if (entry == krep_b200_boyer_moore_search) algo = KREP_B200_ALGO_BMH;
@@ -1370,23 +1757,84 @@ int krep_b200_search_batch(search_func_t entry, const search_params_t *params, c
     else if (entry == krep_b200_simd_avx512_search) algo = KREP_B200_ALGO_AVX512;
     else if (entry == krep_b200_aho_corasick_search) algo = KREP_B200_ALGO_AC;
     else if (entry == krep_b200_neon_search) algo = KREP_B200_ALGO_NEON;
-    if (entry == krep_b200_regex_search)
-    {
-        set_error(-3, "krep_b200_search_batch: regex searches are batched by krep_b200_regex_search_batch");
-        return -3;
-    }
-    if (algo < 0)
-    {
-        set_error(-3, "krep_b200_search_batch: entry must be one of this library's search_func_t entry points");
-        return -3;
-    }
+    if (entry == krep_b200_regex_search) set_error(-3, "%s: regex searches are batched by %s", who, regex_batch);
+    else if (algo < 0) set_error(-3, "%s: entry must be one of this library's search_func_t entry points", who);
+    return algo;
+}
+
+int krep_b200_search_batch(search_func_t entry, const search_params_t *params, const char *const *texts, const size_t *lens,
+                           size_t n_texts, uint64_t *counts, match_result_t *const *results)
+{
+    const int algo = batch_entry_algo(entry, "krep_b200_search_batch", "krep_b200_regex_search_batch");
+    if (algo < 0) return -3;
     return run_batch(algo, params, texts, lens, n_texts, counts, results);
 }
 
-int krep_b200_regex_search_batch(const search_params_t *params, const char *const *texts, const size_t *lens, size_t n_texts,
-                                 uint64_t *counts, match_result_t *const *results)
+int krep_b200_search_batch_resident(search_func_t entry, const search_params_t *params, const void *d_base, const uint64_t *offsets,
+                                    const size_t *lens, size_t n_texts, uint64_t *counts, match_result_t *const *results)
 {
-    return run_regex_batch(params, texts, lens, n_texts, counts, results);
+    clear_error();
+    for (size_t f = 0; counts && f < n_texts; f++) counts[f] = 0;
+    const int algo = batch_entry_algo(entry, "krep_b200_search_batch_resident", "krep_b200_regex_search_batch_resident");
+    if (algo < 0) return -3;
+    return run_batch_resident(algo, params, d_base, offsets, lens, n_texts, counts, results);
+}
+
+int krep_b200_regex_search_batch_resident(const search_params_t *params, const void *d_base, const uint64_t *offsets,
+                                          const size_t *lens, size_t n_texts, uint64_t *counts, match_result_t *const *results)
+{
+    return run_regex_batch_resident(params, d_base, offsets, lens, n_texts, counts, results);
+}
+
+void krep_b200_batch_resident_stats(float *gather_ms, float *scan_ms, double *resolve_ms)
+{
+    if (gather_ms) *gather_ms = t_resident.gather_ms;
+    if (scan_ms) *scan_ms = t_resident.scan_ms;
+    if (resolve_ms) *resolve_ms = t_resident.resolve_ms;
+}
+
+int64_t krep_b200_batch_gather_raw(const void *base, const uint64_t *offsets, const size_t *lens, size_t n, int gap_kind,
+                                   size_t max_gap, void *dst_host, uint64_t cap)
+{
+    static const char *who = "krep_b200_batch_gather_raw";
+    warm_join();
+    std::lock_guard<std::recursive_mutex> lk(engine_mutex());
+    clear_error();
+    if (!base || (n && (!offsets || !lens)) || (cap && !dst_host) || gap_kind < 0 || gap_kind > 1)
+    {
+        set_error(-3, "%s: bad argument", who);
+        return -3;
+    }
+    const size_t gap = gap_kind == 0 ? max_gap + 16 : 1;
+    const uint8_t fill = gap_kind == 0 ? 0 : '\n';
+    std::vector<size_t> live(n);
+    for (size_t f = 0; f < n; f++) live[f] = f;
+    std::vector<uint64_t> off(n, 0);
+    uint64_t total = 0;
+    DeviceGuard guard;
+    cudaPointerAttributes a;
+    const bool on_device = cudaPointerGetAttributes(&a, base) == cudaSuccess && a.type == cudaMemoryTypeDevice;
+    cudaGetLastError();
+    if (!on_device)
+    {
+        // host texts: the host batch's own pack, for comparison
+        DevCtx *Cp = ctx_primary();
+        if (!Cp) return -1;
+        std::vector<const char *> texts(n);
+        for (size_t f = 0; f < n; f++) texts[f] = (const char *)base + offsets[f];
+        if (pack_texts(*Cp, texts.data(), lens, live, gap, fill, &off, &total) != 0) return -2;
+        if (cap) memcpy(dst_host, Cp->h_batch, std::min<uint64_t>(total, cap));
+        return (int64_t)total;
+    }
+    DevCtx *Cp = resident_ctx(who, base, offsets, lens, n);
+    if (!Cp) return krep_b200_last_error() ? krep_b200_last_error() : -1;
+    const int rc = gather_resident(*Cp, who, base, offsets, lens, live, gap, fill, &off, &total, nullptr);
+    if (rc != 0) return rc;
+    if (cap && total)
+    {
+        CKH(cudaMemcpy(dst_host, Cp->d_gather, std::min<uint64_t>(total, cap), cudaMemcpyDeviceToHost));
+    }
+    return (int64_t)total;
 }
 
 void krep_b200_regex_batch_stats(double *pack_ms, double *resolve_ms)

@@ -169,6 +169,62 @@ uint64_t regex_resolve_rows(const search_params_t *P, const void *const *rows, u
     return resolve_views(P, v, n_rows, n, last_byte, true, res, err); // the part that owns every row
 }
 
+// Each text of a packed batch is resolved alone, as resolve_views resolves a one-shard text: its keys and the parts of the
+// row's segments that lie in it, moved to its own coordinates, replayed over its own length, last byte and -m budget.
+// A segment can run past a text's end (its last line ends at the gap's '\n') or into the next text (lines of two texts
+// that abut across a one-byte gap merge into one segment): only the bytes inside the text are its window.  Every window
+// still starts at a line start, the text's own or its first byte.
+int regex_resolve_batch(const search_params_t *P, const void *row, size_t n_texts, const uint64_t *lo, const size_t *len,
+                        const uint8_t *last, const uint64_t *text_lines, uint64_t *counts, match_result_t *const *res)
+{
+    RowView v;
+    if (!row || !view_row(row, ((const RegexRowHeader *)row)->mode, &v))
+    {
+        set_error(-3, "regex batch: not a regex row");
+        return -3;
+    }
+    const uint64_t mode = v.h->mode, nkeys = v.h->nkeys, nseg = v.h->nseg;
+    const int shift = mode == 2 ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+    std::vector<const char *> bytes(nseg);
+    const char *p = v.bytes;
+    for (uint64_t s = 0; s < nseg; s++)
+    {
+        if (v.segs[s].len_cont & 1)
+        {
+            set_error(-3, "regex batch: a segment runs past the packed buffer");
+            return -3;
+        }
+        bytes[s] = p;
+        p += round16(v.segs[s].len_cont >> 1);
+    }
+    std::vector<uint64_t> keys;
+    std::vector<RegexWindow> win;
+    uint64_t j = 0, s0 = 0;
+    for (size_t i = 0; i < n_texts; i++)
+    {
+        const uint64_t b = lo[i], e = lo[i] + len[i];
+        keys.clear();
+        while (j < nkeys && (v.keys[j] >> shift) < b) j++;
+        for (; j < nkeys && (v.keys[j] >> shift) < e; j++) keys.push_back(v.keys[j] - (b << shift));
+        win.clear();
+        while (s0 < nseg && v.segs[s0].start + (v.segs[s0].len_cont >> 1) <= b) s0++;
+        for (uint64_t s = s0; s < nseg && v.segs[s].start < e; s++)
+        {
+            const uint64_t sb = std::max<uint64_t>(v.segs[s].start, b), se = std::min<uint64_t>(v.segs[s].start + (v.segs[s].len_cont >> 1), e);
+            if (se > sb) win.push_back(RegexWindow{(size_t)(sb - b), bytes[s] + (sb - v.segs[s].start), (size_t)(se - sb)});
+        }
+        match_result_t *r = res ? res[i] : nullptr;
+        const size_t n = len[i];
+        if (mode == 2) counts[i] = replay_regex_matches_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last[i], r);
+        else if (mode == 1)
+            counts[i] = std::min<uint64_t>(text_lines[i] + replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n,
+                                                                                last[i], true, nullptr),
+                                           P->max_count);
+        else counts[i] = replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last[i], true, r);
+    }
+    return 0;
+}
+
 } // namespace kb
 
 using namespace kb;

@@ -98,6 +98,19 @@ def load():
                                                         C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64),
                                                         C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64)]
     L.krep_b200_regex_search_batch_long_raw.restype = C.c_int64
+    L.krep_b200_search_batch_resident.argtypes = [C.c_void_p, C.POINTER(SearchParams), C.c_void_p, C.POINTER(C.c_uint64),
+                                                  C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_uint64),
+                                                  C.POINTER(C.POINTER(MatchResult))]
+    L.krep_b200_search_batch_resident.restype = C.c_int
+    L.krep_b200_regex_search_batch_resident.argtypes = [C.POINTER(SearchParams), C.c_void_p, C.POINTER(C.c_uint64),
+                                                        C.POINTER(C.c_size_t), C.c_size_t, C.POINTER(C.c_uint64),
+                                                        C.POINTER(C.POINTER(MatchResult))]
+    L.krep_b200_regex_search_batch_resident.restype = C.c_int
+    L.krep_b200_batch_resident_stats.argtypes = [C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_double)]
+    L.krep_b200_batch_resident_stats.restype = None
+    L.krep_b200_batch_gather_raw.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_size_t), C.c_size_t, C.c_int,
+                                             C.c_size_t, C.c_void_p, C.c_uint64]
+    L.krep_b200_batch_gather_raw.restype = C.c_int64
     L.krep_b200_scan_shard_begin.argtypes = [C.c_void_p, C.POINTER(Shard), C.c_int, C.c_void_p, C.POINTER(C.c_int)]
     L.krep_b200_scan_shard_begin.restype = C.c_int
     L.krep_b200_scan_shard_end.argtypes = [C.c_int, C.POINTER(DeviceResult)]
@@ -291,6 +304,79 @@ def regex_search_batch(params, texts, with_result=True):
     finally:
         for r in res:
             L.krep_b200_match_result_free(r)
+
+
+def _resident_args(tensor, offsets, lens):
+    """(d_base, offsets array, lens array, n) for a uint8 CUDA tensor (any view) and int sequences or CPU int64 tensors."""
+    if not getattr(tensor, "is_cuda", False) or tensor.dtype.itemsize != 1:
+        raise ValueError("texts must be a uint8 CUDA tensor")
+    offs = [int(x) for x in (offsets.tolist() if hasattr(offsets, "tolist") else offsets)]
+    ls = [int(x) for x in (lens.tolist() if hasattr(lens, "tolist") else lens)]
+    if len(offs) != len(ls):
+        raise ValueError("offsets and lens differ in length")
+    n = len(ls)
+    if any(o < 0 or l < 0 or o + l > tensor.numel() for o, l in zip(offs, ls)):
+        raise ValueError("a text lies outside the tensor")
+    if not tensor.is_contiguous():
+        raise ValueError("the tensor must be contiguous")
+    # the library reads the texts on its own stream: whatever torch has queued that writes them must be done first
+    import torch
+    torch.cuda.current_stream(tensor.device).synchronize()
+    return tensor.data_ptr(), (C.c_uint64 * max(n, 1))(*offs), (C.c_size_t * max(n, 1))(*ls), n
+
+
+def search_batch_resident(func, params, tensor, offsets, lens, with_result=True):
+    """krep_b200_search_batch_resident on texts tensor[offsets[i] : offsets[i] + lens[i]] of a uint8 CUDA tensor.
+    -> [(count, [(start, end), ...]), ...], as search_batch on host copies of the texts."""
+    L = load()
+    base, oarr, larr, n = _resident_args(tensor, offsets, lens)
+    L.krep_b200_set_only_matching(bool(params.only_matching))
+    own_trie = False
+    if func == "aho_corasick" and not params.struct.ac_trie:
+        params.struct.ac_trie = L.krep_b200_ac_trie_build(params.ref())
+        own_trie = True
+    counts = (C.c_uint64 * max(n, 1))()
+    res = [L.krep_b200_match_result_init(16) for _ in range(n)] if with_result else []
+    rarr = (C.POINTER(MatchResult) * max(n, 1))(*res) if with_result else None
+    try:
+        entry = C.cast(getattr(L, SEARCH_ENTRIES[func]), C.c_void_p)
+        rc = L.krep_b200_search_batch_resident(entry, params.ref(), base, oarr, larr, n, counts, rarr)
+        check(L)
+        assert rc == 0, rc
+        return [(int(counts[i]), _positions(res[i]) if with_result else []) for i in range(n)]
+    finally:
+        for r in res:
+            L.krep_b200_match_result_free(r)
+        if own_trie:
+            L.krep_b200_ac_trie_free(params.struct.ac_trie)
+            params.struct.ac_trie = None
+        L.krep_b200_set_only_matching(False)
+
+
+def regex_search_batch_resident(params, tensor, offsets, lens, with_result=True):
+    """krep_b200_regex_search_batch_resident on texts tensor[offsets[i] : offsets[i] + lens[i]] of a uint8 CUDA tensor.
+    -> [(count, [(start, end), ...]), ...], as regex_search_batch on host copies of the texts."""
+    L = load()
+    base, oarr, larr, n = _resident_args(tensor, offsets, lens)
+    counts = (C.c_uint64 * max(n, 1))()
+    res = [L.krep_b200_match_result_init(16) for _ in range(n)] if with_result else []
+    rarr = (C.POINTER(MatchResult) * max(n, 1))(*res) if with_result else None
+    try:
+        rc = L.krep_b200_regex_search_batch_resident(params.ref(), base, oarr, larr, n, counts, rarr)
+        check(L)
+        assert rc == 0, rc
+        return [(int(counts[i]), _positions(res[i]) if with_result else []) for i in range(n)]
+    finally:
+        for r in res:
+            L.krep_b200_match_result_free(r)
+
+
+def batch_resident_stats():
+    """(gather_ms, scan_ms, resolve_ms) of the calling thread's most recent resident batch call."""
+    L = load()
+    g, s, r = C.c_float(), C.c_float(), C.c_double()
+    L.krep_b200_batch_resident_stats(C.byref(g), C.byref(s), C.byref(r))
+    return g.value, s.value, r.value
 
 
 def _positions(res):
