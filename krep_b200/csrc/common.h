@@ -80,6 +80,15 @@ static constexpr uint32_t REGEX_LONG_MAX_MATCH = 8192;      // a match this long
 //   uncertain key : global_line_start << 16
 static constexpr int REGEX_MATCH_SHIFT = 16;
 static constexpr uint64_t REGEX_MATCH_MAX_OFFSET = 1ull << 48;
+// The three modes of k_regex_lines.  The values are the C ABI's `int mode` and RegexRowHeader::mode (DESIGN §12.4).
+enum RegexMode : int
+{
+    RX_FILTER = 0,  // one key per flagged line; glibc confirms them
+    RX_COUNT = 1,   // fused -c: lines decided MATCHED are counted, uncertain lines leave keys
+    RX_OFFSETS = 2, // offsets: one key per match of a line decided MATCHED, uncertain lines leave keys
+};
+// Where a mode's keys hold the line or match start: LIT_TAG_BITS, or REGEX_MATCH_SHIFT in the offsets mode.
+inline int regex_key_shift(RegexMode mode) { return mode == RX_OFFSETS ? REGEX_MATCH_SHIFT : LIT_TAG_BITS; }
 // The anchored match automaton shares the kernel's default dynamic shared memory with the line table and the class map.
 static constexpr uint32_t REGEX_SMEM_BYTES = 48 * 1024;
 // Enumeration budget of one line in match mode: automaton steps (plus one per start position tried) before the line is
@@ -107,6 +116,11 @@ struct RegexDfa
     // the three flags above (the union's); a plan of one automaton leaves it empty.
     std::vector<RegexDfa> groups;
 };
+// Is `mode` (any int, as the C ABI passes it) one the plan of D can run?  The count and offsets modes need the exact flags.
+inline bool regex_mode_available(const RegexDfa &D, int mode)
+{
+    return mode == RX_FILTER || (mode == RX_COUNT && D.count_exact) || (mode == RX_OFFSETS && D.offsets_exact);
+}
 static constexpr uint16_t RX_ACC = 1, RX_ACC_EOL = 2;
 // Padded size in 16-bit words of the table image the kernel copies to shared memory: line table, class map, match table.
 __host__ __device__ inline uint32_t regex_tab_words(uint32_t ntrans) { return (ntrans + 7) & ~7u; }
@@ -165,7 +179,7 @@ static constexpr uint64_t ROW_LAST_BYTE_SHIFT = 8;
 struct RegexRowHeader
 {
     uint64_t magic;
-    uint64_t mode;         // 0 filter, 1 count (fused -c), 2 match (offsets on the device)
+    uint64_t mode;         // RegexMode
     uint64_t row_bytes;    // the whole row, a multiple of 16
     uint64_t device_lines; // count mode: lines of the shard decided MATCHED on the device
     uint64_t nkeys, nseg, head_len;
@@ -370,6 +384,18 @@ uint64_t replay_regex_windows(const search_params_t *P, const uint64_t *keys, si
                               size_t n, int last_byte, bool at_end, match_result_t *res);
 uint64_t replay_regex_matches_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w,
                                       size_t nw, size_t n, int last_byte, match_result_t *res);
+// The -E call is answered 0 before the text is looked at: -m 0 with -c or positions (krep.c:1395), or no compiled regex
+// (krep.c:1399).
+bool regex_returns_early(const search_params_t *P);
+// The answer on an empty text (krep.c:1403-1416) of a call that did not return early: whether the regex matches the
+// empty string.
+uint64_t regex_empty_text(const search_params_t *P, match_result_t *res);
+// The answer of a -E call from the keys of a scan in `mode`; device_lines: the lines the count mode decided MATCHED.
+uint64_t regex_answer(const search_params_t *P, RegexMode mode, uint64_t device_lines, const Replay &r, match_result_t *res);
+// The same over windows of the text (replay_regex_windows); at_end: the filter and count modes decide the empty string
+// at n after the last window.
+uint64_t regex_answer_windows(const search_params_t *P, RegexMode mode, uint64_t device_lines, const std::vector<uint64_t> &keys,
+                              const std::vector<RegexWindow> &w, size_t n, int last_byte, bool at_end, match_result_t *res);
 // regex_rows.cpp: the answer of a -E search from the rows of the shards that tile the text (text order).  *err: 0, or
 // -3 with the error set.
 uint64_t regex_resolve_rows(const search_params_t *P, const void *const *rows, uint32_t n_rows, match_result_t *res, int *err);

@@ -252,6 +252,15 @@ DevCtx *ctx_primary()
     return d < 0 ? nullptr : ctx_get(d);
 }
 
+// a single process may hold shards on several GPUs; a failed lookup's error is cleared
+DevCtx *ctx_of_pointer(const void *d_ptr)
+{
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, d_ptr) == cudaSuccess && a.type == cudaMemoryTypeDevice) return ctx_get(a.device);
+    cudaGetLastError();
+    return ctx_primary();
+}
+
 static std::vector<Plan *> g_all_plans; // every live plan (device copies are released at shutdown)
 static std::mutex g_plans_mu;
 
@@ -828,9 +837,9 @@ static int bits_for(uint64_t v)
     return b;
 }
 
-int key_end_bit(const Plan *plan, uint64_t max_offset, bool regex_matches)
+int key_end_bit(const Plan *plan, uint64_t max_offset, RegexMode mode)
 {
-    const int shift = plan->is_ac ? AC_END_SHIFT : regex_matches ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+    const int shift = plan->is_ac ? AC_END_SHIFT : regex_key_shift(mode);
     int b = bits_for(max_offset) + shift;
     return b > 64 ? 64 : b;
 }
@@ -1185,15 +1194,6 @@ const char *krep_b200_plan_filter_name(const krep_b200_plan_t *plan)
     return plan ? reinterpret_cast<const Plan *>(plan)->filter_name.c_str() : "";
 }
 
-// the context of the device that owns a device pointer (a single process may hold shards on several GPUs)
-static DevCtx *ctx_of_pointer(const void *d_ptr)
-{
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, d_ptr) == cudaSuccess && a.type == cudaMemoryTypeDevice) return ctx_get(a.device);
-    cudaGetLastError();
-    return ctx_primary();
-}
-
 static void fill_result(const ScanOut &so, const krep_b200_shard_t *shard, int slot, krep_b200_device_result_t *out)
 {
     out->count = so.count;
@@ -1262,12 +1262,12 @@ int krep_b200_scan_shard(const krep_b200_plan_t *plan, const krep_b200_shard_t *
 
 } // extern "C"
 
-// One k_regex_lines scan of a shard in the given mode (0 filter, 1 count, 2 match) on the device's scan stream, its keys
-// sorted on the device: *d_sorted (device, *cnt keys; short lists sorted by k_finish into d_pack, longer ones by the radix
-// sort, enqueued on the stream) and the count mode's line counter.  Unlike scan_end's retry, an overflow re-scan keeps the
+// One k_regex_lines scan of a shard in the given mode on the device's scan stream, its keys sorted on the device:
+// *d_sorted (device, *cnt keys; short lists sorted by k_finish into d_pack, longer ones by the radix sort, enqueued on
+// the stream) and the count mode's line counter.  Unlike scan_end's retry, an overflow re-scan keeps the
 // mode and zeroes the line counter again, so the keys and the count are those of one complete scan.  The lists stay valid
 // until the next scan on the device.  long_lines: the long-line pass follows the scan (DESIGN §12.8).
-int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt_out,
+int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, RegexMode mode, const char *who, uint64_t *cnt_out,
                         const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines, const RegexBatchDev *batch)
 {
     for (int s = 0; s < SCAN_SLOTS; s++)
@@ -1277,8 +1277,8 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
             return -3;
         }
     const uint64_t n_lines = batch ? batch->n_texts : 1; // line counters: one per text of a batch
-    if (ensure_keys(E, 1) != 0 || (mode == 1 && ensure_line_out(E, (n_lines + 1) / 2) != 0)) return -2;
-    unsigned long long *d_lines = mode == 1 ? (unsigned long long *)E.d_line_out : nullptr;
+    if (ensure_keys(E, 1) != 0 || (mode == RX_COUNT && ensure_line_out(E, (n_lines + 1) / 2) != 0)) return -2;
+    unsigned long long *d_lines = mode == RX_COUNT ? (unsigned long long *)E.d_line_out : nullptr;
     const int slot = 0;
     cudaStream_t st = E.scan_stream;
     ++E.serial; // slot 0's lists are overwritten: a device result handed out earlier no longer passes the stale check
@@ -1287,7 +1287,7 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
         CK(cudaStreamWaitEvent(st, E.ev_done[slot], 0));
         if (reset_counter(E, slot, st) != 0) return -2;
         if (d_lines) CK(cudaMemsetAsync(d_lines, 0, n_lines * sizeof(unsigned long long), st));
-        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == 2, batch, long_lines);
+        int rc = launch_scan(E, plan, shard, 1, st, slot, d_lines, mode == RX_OFFSETS, batch, long_lines);
         if (rc != 0) return rc;
         if (finish_scan(E, slot, 1, st) != 0) return -2;
         if (d_lines) CK(cudaMemcpyAsync(E.h_line_out, d_lines, n_lines * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -1301,7 +1301,7 @@ int kb::regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *sh
         *d_sorted = E.d_pack[slot] + 1;
         if (cnt > PACK_KEYS)
         {
-            rc = sort_keys(E, slot, cnt, key_end_bit(plan, shard->global_offset + shard->avail_len, mode == 2), st, d_sorted);
+            rc = sort_keys(E, slot, cnt, key_end_bit(plan, shard->global_offset + shard->avail_len, mode), st, d_sorted);
             if (rc != 0) return rc;
         }
         *cnt_out = cnt;
@@ -1328,7 +1328,7 @@ static int64_t regex_scan_raw(const char *who, const krep_b200_plan_t *plan_, co
         set_error(-3, "%s: null argument", who);
         return -3;
     }
-    if (!plan->is_regex || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    if (!plan->is_regex || !regex_mode_available(*plan->rx, mode))
     {
         set_error(-3, "%s: mode %d is not available for this plan", who, mode);
         return -3;
@@ -1339,7 +1339,7 @@ static int64_t regex_scan_raw(const char *who, const krep_b200_plan_t *plan_, co
     DevCtx &E = *Cp;
     uint64_t cnt = 0;
     const uint64_t *d_sorted = nullptr;
-    const int rc = regex_scan_keys(E, plan, shard, mode, who, &cnt, &d_sorted, device_lines, long_lines);
+    const int rc = regex_scan_keys(E, plan, shard, (RegexMode)mode, who, &cnt, &d_sorted, device_lines, long_lines);
     if (rc != 0) return rc;
     const uint64_t n = cnt < cap ? cnt : cap;
     if (cnt <= PACK_KEYS)

@@ -103,7 +103,7 @@ struct RegexPackStats
 // One k_regex_lines scan of the shard in `mode` with its keys sorted on the device (engine.cu); long_lines: followed by
 // the long-line pass (nullptr: not).  batch: the shard is a packed -E batch with this text table, scanned in the
 // kernel's batch mode; the count mode then leaves one line count per text in device_lines[0 .. batch->n_texts).
-int regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, int mode, const char *who, uint64_t *cnt,
+int regex_scan_keys(DevCtx &E, const Plan *plan, const krep_b200_shard_t *shard, RegexMode mode, const char *who, uint64_t *cnt,
                     const uint64_t **d_sorted, uint64_t *device_lines, const LongLineOpts *long_lines = nullptr,
                     const RegexBatchDev *batch = nullptr);
 // Packs the row of the shard whose sorted keys (nkeys, in `mode`'s layout) are at d_keys into engine-owned device memory
@@ -132,6 +132,7 @@ int primary_device();            // device bound by krep_b200_init, else the cal
 int visible_devices();           // cudaGetDeviceCount (0 when CUDA is unusable)
 DevCtx *ctx_get(int device);     // creates the context on first use; nullptr after set_error
 DevCtx *ctx_primary();           // ctx_get(primary_device())
+DevCtx *ctx_of_pointer(const void *d_ptr); // the context of the device that owns d_ptr, else ctx_primary()
 void engine_shutdown();
 void prewarm_host_path(DevCtx &C); // host_api.cu: rings + occurrence list for the pageable-text path
 void keep_devices_visible(); // the host manages devices itself: do not narrow CUDA_VISIBLE_DEVICES
@@ -161,7 +162,7 @@ int finish_scan(DevCtx &C, int slot, int want_sort, cudaStream_t stream, bool ke
 int ensure_keys(DevCtx &C, uint64_t cap);
 int reset_counter(DevCtx &C, int slot, cudaStream_t stream);
 int sort_keys(DevCtx &C, int slot, uint64_t n, int end_bit, cudaStream_t stream, const uint64_t **sorted);
-int key_end_bit(const Plan *plan, uint64_t max_offset, bool regex_matches = false); // regex_matches: match-mode keys
+int key_end_bit(const Plan *plan, uint64_t max_offset, RegexMode mode = RX_FILTER); // mode: of a regex plan's keys
 int fetch_keys(DevCtx &C, const ScanOut &so, const uint64_t **h); // sorted keys on the host (no copy when they came back packed)
 void add_kernel_ms(float ms);
 void reset_kernel_ms();

@@ -147,6 +147,23 @@ static Plan *cached_regex_plan(const search_params_t *P, std::string *why)
     return pl;
 }
 
+// cached_regex_plan without the reason; nullptr for null params too
+static Plan *regex_plan_of(const search_params_t *P)
+{
+    std::string why;
+    return P ? cached_regex_plan(P, &why) : nullptr;
+}
+
+// The plan a -E call runs, or nullptr with the error set when the compiler refused the pattern.
+static Plan *regex_plan_or_refuse(const search_params_t *P)
+{
+    std::string why;
+    Plan *plan = cached_regex_plan(P, &why);
+    if (!plan)
+        set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
+    return plan;
+}
+
 void plan_cache_clear()
 {
     g_regex_refusals.clear();
@@ -358,12 +375,12 @@ struct RangeJob
     size_t n = 0, begin = 0, end = 0, chunk = 0;
     int want_positions = 0;
     bool pinned = false;
-    bool count_lines = false; // fused -c: every chunk leaves one line record instead of occurrence keys
+    bool count_lines = false; // fused -c of a literal or pattern-set plan: every chunk leaves one line record instead of keys
     std::vector<uint64_t> line_recs; // (lines, flags) per chunk, text order
-    bool regex_count = false; // fused -E -c: every chunk adds its device-decided matching lines and leaves its uncertain keys
+    // -E: the scan's mode.  RX_COUNT: every chunk adds its device-decided matching lines and leaves its uncertain keys
+    RegexMode regex_mode = RX_FILTER;
     uint64_t regex_lines = 0; // lines of the range decided MATCHED on the device
-    bool regex_matches = false; // -E offsets on the device: match keys and uncertain-line keys (REGEX_MATCH_SHIFT layout)
-    const RegexBatch *batch = nullptr; // -E batch: the text is packed texts; regex_count then counts per text
+    const RegexBatch *batch = nullptr; // -E batch: the text is packed texts; RX_COUNT then counts per text
     const LongLineOpts *long_lines = nullptr; // -E: the long-line pass after each chunk's scan (DESIGN §12.8)
     std::vector<uint64_t> text_lines;  // batch, fused -c: lines of each text decided MATCHED in this range
     // results
@@ -393,8 +410,9 @@ static int stream_range(RangeJob &J)
     if (J.count_lines && ensure_line_out(E, nchunks) != 0) return -2;
     // the range's line counter: d_line_out[0] (a batch: one per text, d_line_out[0 .. n_texts))
     const size_t n_lines = J.batch ? J.batch->end.size() : 1;
-    if (J.regex_count && ensure_line_out(E, (n_lines + 1) / 2) != 0) return -2;
-    unsigned long long *d_regex_lines = J.regex_count ? (unsigned long long *)E.d_line_out : nullptr;
+    const bool regex_count = J.regex_mode == RX_COUNT;
+    if (regex_count && ensure_line_out(E, (n_lines + 1) / 2) != 0) return -2;
+    unsigned long long *d_regex_lines = regex_count ? (unsigned long long *)E.d_line_out : nullptr;
     RegexBatchDev batch_dev{};
     if (J.batch && upload_regex_batch(E, *J.batch, &batch_dev) != 0) return -2;
     reset_kernel_ms();
@@ -454,7 +472,7 @@ static int stream_range(RangeJob &J)
             else
                 rc = J.count_lines ? launch_count_lines(E, plan, &part, E.scan_stream, c)
                                    : launch_scan(E, plan, &part, J.want_positions, E.scan_stream, slot, d_regex_lines,
-                                                 J.regex_matches, J.batch ? &batch_dev : nullptr, J.long_lines);
+                                                 J.regex_mode == RX_OFFSETS, J.batch ? &batch_dev : nullptr, J.long_lines);
             if (rc != 0) return rc;
             CKH(cudaEventRecord(b, E.scan_stream));
             if (!set_count) CKH(cudaEventRecord(E.ring_scanned[rs], E.scan_stream));
@@ -484,8 +502,8 @@ static int stream_range(RangeJob &J)
             J.so = ScanOut();
             return 0;
         }
-        if (J.regex_count && J.batch) J.text_lines.assign(E.h_line_out, E.h_line_out + n_lines);
-        else if (J.regex_count) J.regex_lines = E.h_line_out[0];
+        if (regex_count && J.batch) J.text_lines.assign(E.h_line_out, E.h_line_out + n_lines);
+        else if (regex_count) J.regex_lines = E.h_line_out[0];
         const uint64_t cnt = E.h_pack[slot][0];
         J.so = ScanOut();
         J.so.count = cnt;
@@ -502,7 +520,7 @@ static int stream_range(RangeJob &J)
                 J.so.h_sorted = E.h_pack[slot] + 1;
                 return 0;
             }
-            return sort_keys(E, slot, cnt, key_end_bit(plan, n, J.regex_matches), E.scan_stream, &J.so.d_keys);
+            return sort_keys(E, slot, cnt, key_end_bit(plan, n, J.regex_mode), E.scan_stream, &J.so.d_keys);
         }
         // list overflowed: grow it and stage the range again (the ring holds only the last chunks)
         J.so.overflow = 1;
@@ -553,12 +571,12 @@ struct HostScan
     std::vector<uint64_t> text_lines; // the same per text of a batch
 };
 
-// count_lines: the fused -c of the plan — a line record per chunk for literals; for regex plans a device line count per
-// range next to the keys of the uncertain lines (want_positions must then be set).  regex_matches: -E offsets on the
-// device (offsets_exact regex plans, want_positions set): the keys are match keys and uncertain-line keys.  batch: the
-// text is a packed -E batch with this text table (DESIGN §12.5).
+// count_lines: the fused -c of a literal or pattern-set plan, a line record per chunk.  regex_mode: the k_regex_lines
+// mode of a regex plan (want_positions set): RX_COUNT leaves a device line count per range next to the keys of the
+// uncertain lines, RX_OFFSETS match keys and uncertain-line keys.  batch: the text is a packed -E batch with this text
+// table (DESIGN §12.5).
 static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want_positions, HostScan *hs, bool count_lines = false,
-                          bool regex_matches = false, const RegexBatch *batch = nullptr)
+                          RegexMode regex_mode = RX_FILTER, const RegexBatch *batch = nullptr)
 {
     const bool pinned = is_pinned(text);
     const size_t chunk = pinned ? env_mb("KREP_B200_CHUNK_MB", 256) : env_mb("KREP_B200_STAGE_MB", 32);
@@ -589,9 +607,8 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
         J.end = std::min((i + 1) * per * chunk, n);
         J.want_positions = want_positions;
         J.pinned = pinned;
-        J.count_lines = count_lines && !plan->is_regex;
-        J.regex_count = count_lines && plan->is_regex;
-        J.regex_matches = regex_matches;
+        J.count_lines = count_lines;
+        J.regex_mode = regex_mode;
         J.batch = batch;
         J.long_lines = !plan->is_regex ? nullptr : batch ? batch->long_lines : long_lines_default();
     }
@@ -660,14 +677,14 @@ static int stage_and_scan(const Plan *plan, const char *text, size_t n, int want
     hs->nkeys = 0;
     hs->regex_lines = 0;
     hs->text_lines.clear();
-    if (batch && count_lines)
+    if (batch && regex_mode == RX_COUNT)
     {
         // every line is decided by one range: the per-text counts add up
         hs->text_lines.assign(batch->end.size(), 0);
         for (auto &J : jobs)
             for (size_t i = 0; i < J.text_lines.size(); i++) hs->text_lines[i] += J.text_lines[i];
     }
-    if (count_lines && !plan->is_regex)
+    if (count_lines)
     {
         // chunk records of all ranges, in text order -> matching lines (a line cut by a chunk / range / device edge is
         // counted on both sides and subtracted once)
@@ -882,22 +899,6 @@ static bool regex_count_fused(const search_params_t *P, const Plan *plan)
     return regex_count_exact(P, plan) && !getenv("KREP_B200_NO_FUSED_COUNT");
 }
 
-// Fused -E -c: the answer is  min(lines the device decided MATCHED + replay_regex over the uncertain lines, max_count).
-// Why this is the reference's count: without -w and -o the loop of krep.c:1389-1579 calls regexec only at line starts
-// (after a counted line the cursor jumps to the next line start; with no match left the loop ends) and never with
-// REG_NOTBOL, and under REG_NEWLINE no match contains a '\n'.  So a line is counted exactly when glibc finds a match in
-// it from its start, each line independently of the others — which the automaton of a count_exact plan decides — and
-// the -m limit only caps the total.  Two answers depend on the end of the text rather than on one line: '$' cannot
-// match at the end of the text under -i (REG_ICASE passed as an execution flag is REG_NOTEOL), and a text that ends in
-// '\n' holds an empty string at n that is counted when the last line was not and the regex matches there.  The line
-// holding the text's last byte is always among the uncertain keys, so both are decided inside glibc's last run, as in
-// the reference; skipping the lines counted on the device changes nothing for the runs in between, since each run starts
-// at a line start.
-static uint64_t regex_count_total(const search_params_t *P, uint64_t device_lines, const Replay &uncertain)
-{
-    return std::min<uint64_t>(device_lines + replay_regex(P, uncertain, nullptr), P->max_count);
-}
-
 // Can a -E call with these params compute its match offsets on the device?  Positions or -co (track_positions without
 // count_lines_mode), no -w, on a plan whose match automaton is exact and fits (offsets_exact).
 // KREP_B200_NO_DEVICE_MATCHES is not looked at here.
@@ -911,21 +912,24 @@ static bool regex_matches_device(const search_params_t *P, const Plan *plan)
     return regex_matches_exact(P, plan) && !getenv("KREP_B200_NO_DEVICE_MATCHES");
 }
 
+// The k_regex_lines mode a -E call with these params takes.
+static RegexMode regex_call_mode(const search_params_t *P, const Plan *plan)
+{
+    return regex_count_fused(P, plan) ? RX_COUNT : regex_matches_device(P, plan) ? RX_OFFSETS : RX_FILTER;
+}
+
 // -E (regex_search, krep.c:1389): the device flags the lines the regex can match in (k_regex_lines), glibc's regexec
 // on the caller's regex_t confirms them and computes every offset (replay_regex).  A -c call on a count_exact plan
-// counts the lines the device can decide there and leaves glibc only the uncertain ones (regex_count_total).  A
-// positions or -co call on an offsets_exact plan takes the offsets of the lines the device decides from the device and
-// leaves glibc only the uncertain ones (replay_regex_matches, DESIGN §12.2).  The empty text is answered on the host,
-// as the reference does, without a launch.
+// counts the lines the device can decide there and leaves glibc only the uncertain ones.  A positions or -co call on an
+// offsets_exact plan takes the offsets of the lines the device decides from the device and leaves glibc only the
+// uncertain ones (DESIGN §12.2).  regex_answer turns each mode's keys into the answer.  The empty text is answered on
+// the host, as the reference does, without a launch.
 static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, match_result_t *res)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
     clear_error();
-    if (!P) return 0;
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
-    Replay r{nullptr, 0, text, n, 0};
-    if (n == 0) return replay_regex(P, r, res); // krep.c:1403-1416
+    if (!P || regex_returns_early(P)) return 0;
+    if (n == 0) return regex_empty_text(P, res);
     if (!text) return 0;
     warm_join();
     if (visible_devices() == 0)
@@ -934,45 +938,19 @@ static uint64_t run_regex(const search_params_t *P, const char *text, size_t n, 
         return 0;
     }
     DeviceGuard guard;
-    std::string why;
-    Plan *plan = cached_regex_plan(P, &why);
-    if (!plan)
-    {
-        set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
-        return 0;
-    }
-    const bool fused = regex_count_fused(P, plan);
-    const bool matches = !fused && regex_matches_device(P, plan);
+    Plan *plan = regex_plan_or_refuse(P);
+    if (!plan) return 0;
+    const RegexMode mode = regex_call_mode(P, plan);
     HostScan hs;
-    if (stage_and_scan(plan, text, n, 1, &hs, fused, matches) != 0) return 0;
-    r.keys = hs.keys;
-    r.n = (size_t)hs.nkeys;
-    if (matches)
-    {
-        const uint64_t ret = replay_regex_matches(P, r, res);
-        trace("search: regex offsets on the device: %llu keys (%llu)", (unsigned long long)hs.nkeys, (unsigned long long)ret);
-        return ret;
-    }
-    if (fused)
-    {
-        const uint64_t ret = regex_count_total(P, hs.regex_lines, r);
-        trace("search: regex -c fused: %llu lines counted on the device, %llu uncertain lines to regexec (%llu)",
-              (unsigned long long)hs.regex_lines, (unsigned long long)hs.nkeys, (unsigned long long)ret);
-        return ret;
-    }
-    const uint64_t ret = replay_regex(P, r, res);
-    trace("search: regex confirmed on %llu flagged lines (%llu)", (unsigned long long)hs.nkeys, (unsigned long long)ret);
+    if (stage_and_scan(plan, text, n, 1, &hs, false, mode) != 0) return 0;
+    const uint64_t ret = regex_answer(P, mode, hs.regex_lines, Replay{hs.keys, (size_t)hs.nkeys, text, n, 0}, res);
+    trace("search: regex mode %d: %llu keys to regexec or offsets, %llu lines counted on the device (%llu)", mode,
+          (unsigned long long)hs.nkeys, (unsigned long long)hs.regex_lines, (unsigned long long)ret);
     return ret;
 }
 
 // ---- -E on resident shards (DESIGN §12.4): a row per shard, resolved on the host ----
 static thread_local RegexPackStats t_rx_stats; // of the most recent krep_b200_search_shards / _regex_export_shard call
-
-// The k_regex_lines mode a -E call with these params takes, as in run_regex: 1 = fused -c, 2 = offsets, 0 = filter.
-static int regex_call_mode(const search_params_t *P, const Plan *plan)
-{
-    return regex_count_fused(P, plan) ? 1 : regex_matches_device(P, plan) ? 2 : 0;
-}
 
 // Scan + pack of one shard: the row is left in the engine's memory of the shard's device.
 static int regex_export(const Plan *plan, const search_params_t *P, const krep_b200_shard_t *sh, const char *who, DevCtx **ctx,
@@ -983,12 +961,10 @@ static int regex_export(const Plan *plan, const search_params_t *P, const krep_b
         set_error(-3, "%s: not a regex plan", who);
         return -3;
     }
-    cudaPointerAttributes a;
-    DevCtx *C = (cudaPointerGetAttributes(&a, sh->d_text) == cudaSuccess && a.type == cudaMemoryTypeDevice) ? ctx_get(a.device) : ctx_primary();
-    cudaGetLastError();
+    DevCtx *C = ctx_of_pointer(sh->d_text);
     if (!C) return -1;
     cudaSetDevice(C->device);
-    const int mode = regex_call_mode(P, plan);
+    const RegexMode mode = regex_call_mode(P, plan);
     uint64_t cnt = 0, lines = 0;
     const uint64_t *d_sorted = nullptr;
     CKH(cudaEventRecord(C->ev_ca, C->scan_stream));
@@ -1033,10 +1009,9 @@ static uint64_t search_shards_regex(const Plan *plan, const search_params_t *P, 
                       "offset 0 with prev_byte -1, owned ranges abut, the last has next_byte -1 and own_end == avail_len");
         return 0;
     }
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    if (regex_returns_early(P)) return 0;
     const krep_b200_shard_t &last = shards[n_shards - 1];
-    if (last.global_offset + last.avail_len == 0) return replay_regex(P, Replay{nullptr, 0, nullptr, 0, 0}, res); // krep.c:1403
+    if (last.global_offset + last.avail_len == 0) return regex_empty_text(P, res);
     DeviceGuard guard;
     std::vector<std::vector<uint8_t>> copies(n_shards > 1 ? n_shards : 0);
     std::vector<const void *> rows(n_shards);
@@ -1254,14 +1229,14 @@ static void regex_batch_table(const size_t *lens, const std::vector<size_t> &liv
     }
 }
 
-// One k_regex_lines scan in `mode` (0 filter, 1 fused -c, 2 offsets) of the texts f in `live` (ascending, lens[f] > 0):
-// packed with '\n' gaps (at least one '\n' after each text, up to the next 16-byte boundary), so that no line and no
-// automaton walk crosses from one text into the next, and scanned by stage_and_scan as one text in the kernel's batch
-// mode.  *off (indexed by f): packed offsets; *hs: the sorted keys in packed coordinates and, in mode 1, the device line
-// count of each live text (indexed like `live`).  long_lines: the long-line pass after each chunk's scan, in the batch
+// One k_regex_lines scan in `mode` of the texts f in `live` (ascending, lens[f] > 0): packed with '\n' gaps (at least
+// one '\n' after each text, up to the next 16-byte boundary), so that no line and no automaton walk crosses from one
+// text into the next, and scanned by stage_and_scan as one text in the kernel's batch mode.  *off (indexed by f):
+// packed offsets; *hs: the sorted keys in packed coordinates and, in RX_COUNT, the device line count of each live text
+// (indexed like `live`).  long_lines: the long-line pass after each chunk's scan, in the batch
 // rules (DESIGN §12.8); nullptr leaves every line past the kernel's reach uncertain.
 static int regex_batch_scan(const Plan *plan, const char *const *texts, const size_t *lens, const std::vector<size_t> &live,
-                            int mode, const LongLineOpts *long_lines, const char *who, std::vector<uint64_t> *off, HostScan *hs)
+                            RegexMode mode, const LongLineOpts *long_lines, const char *who, std::vector<uint64_t> *off, HostScan *hs)
 {
     if (live.size() >= UINT32_MAX)
     {
@@ -1278,7 +1253,7 @@ static int regex_batch_scan(const Plan *plan, const char *const *texts, const si
     regex_batch_table(lens, live, *off, total, &B);
     t_rx_batch.pack_ms += ms_since(t0);
     trace("regex batch: %zu texts packed into %llu bytes", live.size(), (unsigned long long)total);
-    return stage_and_scan(plan, (const char *)Cp->h_batch, total, 1, hs, mode == 1, mode == 2, &B);
+    return stage_and_scan(plan, (const char *)Cp->h_batch, total, 1, hs, false, mode, &B);
 }
 
 // krep_b200_regex_search_batch: text i gets krep_b200_regex_search(P, texts[i], lens[i], results[i])'s answer.  The
@@ -1298,8 +1273,7 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
         return -3;
     }
     for (size_t f = 0; f < nt; f++) counts[f] = 0;
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    if (regex_returns_early(P)) return 0;
     std::vector<size_t> live;
     for (size_t f = 0; f < nt; f++)
         if (lens[f] > 0 && texts[f]) live.push_back(f);
@@ -1311,21 +1285,16 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
             set_error(-1, "no CUDA device available; this engine has no CPU fallback");
             return -1;
         }
-        std::string why;
-        Plan *plan = cached_regex_plan(P, &why);
-        if (!plan)
-        {
-            set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
-            return -3;
-        }
-        const int mode = regex_call_mode(P, plan);
+        Plan *plan = regex_plan_or_refuse(P);
+        if (!plan) return -3;
+        const RegexMode mode = regex_call_mode(P, plan);
         std::vector<uint64_t> off(nt, 0);
         HostScan hs;
         const int rc = regex_batch_scan(plan, texts, lens, live, mode, long_lines_default(), "krep_b200_regex_search_batch", &off, &hs);
         if (rc != 0) return rc;
         const auto t0 = std::chrono::steady_clock::now();
         // keys ascend in packed coordinates: one pass cuts them per text (nothing outside a text is kept)
-        const int shift = mode == 2 ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+        const int shift = regex_key_shift(mode);
         size_t j = 0;
         for (size_t i = 0; i < live.size(); i++)
         {
@@ -1335,8 +1304,7 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
             size_t k = j;
             while (k < hs.nkeys && (hs.keys[k] >> shift) < hi) k++;
             const Replay r{hs.keys + j, k - j, texts[f], lens[f], lo};
-            match_result_t *res = results ? results[f] : nullptr;
-            counts[f] = mode == 2 ? replay_regex_matches(P, r, res) : mode == 1 ? regex_count_total(P, hs.text_lines[i], r) : replay_regex(P, r, res);
+            counts[f] = regex_answer(P, mode, mode == RX_COUNT ? hs.text_lines[i] : 0, r, results ? results[f] : nullptr);
             j = k;
         }
         t_rx_batch.resolve_ms = ms_since(t0);
@@ -1344,7 +1312,7 @@ static int run_regex_batch(const search_params_t *P, const char *const *texts, c
               t_rx_batch.resolve_ms);
     }
     for (size_t f = 0; f < nt; f++)
-        if (lens[f] == 0) counts[f] = replay_regex(P, Replay{nullptr, 0, texts[f], 0, 0}, results ? results[f] : nullptr); // krep.c:1403
+        if (lens[f] == 0) counts[f] = regex_empty_text(P, results ? results[f] : nullptr);
     return 0;
 }
 
@@ -1615,26 +1583,20 @@ static int run_regex_batch_resident(const search_params_t *P, const void *d_base
     DevCtx *Cp = resident_ctx(who, d_base, offsets, lens, nt);
     if (!Cp) return krep_b200_last_error() ? krep_b200_last_error() : -1;
     DevCtx &E = *Cp;
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    if (regex_returns_early(P)) return 0;
     std::vector<size_t> live;
     for (size_t f = 0; f < nt; f++)
         if (lens[f] > 0) live.push_back(f);
     if (!live.empty())
     {
-        std::string why;
-        Plan *plan = cached_regex_plan(P, &why);
-        if (!plan)
-        {
-            set_error(-3, "this regex is not run on the GPU (%s); krep_b200_select_search_algorithm returns NULL for it", why.c_str());
-            return -3;
-        }
+        Plan *plan = regex_plan_or_refuse(P);
+        if (!plan) return -3;
         if (live.size() >= UINT32_MAX)
         {
             set_error(-3, "%s: too many texts in one call", who);
             return -3;
         }
-        const int mode = regex_call_mode(P, plan);
+        const RegexMode mode = regex_call_mode(P, plan);
         const size_t nl = live.size();
         std::vector<uint64_t> off(nt, 0);
         std::vector<uint8_t> last;
@@ -1681,7 +1643,7 @@ static int run_regex_batch_resident(const search_params_t *P, const void *d_base
               (unsigned long long)row_bytes, t_resident.resolve_ms);
     }
     for (size_t f = 0; f < nt; f++)
-        if (lens[f] == 0) counts[f] = replay_regex(P, Replay{nullptr, 0, "", 0, 0}, results ? results[f] : nullptr); // krep.c:1403
+        if (lens[f] == 0) counts[f] = regex_empty_text(P, results ? results[f] : nullptr);
     return 0;
 }
 
@@ -1856,9 +1818,8 @@ static int64_t regex_batch_raw(const char *who, const search_params_t *P, const 
         set_error(-3, "%s: null argument", who);
         return -3;
     }
-    std::string why;
-    Plan *plan = cached_regex_plan(P, &why);
-    if (!plan || mode < 0 || mode > 2 || (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    Plan *plan = regex_plan_of(P);
+    if (!plan || !regex_mode_available(*plan->rx, mode))
     {
         set_error(-3, "%s: mode %d is not available for this pattern", who, mode);
         return -3;
@@ -1874,12 +1835,12 @@ static int64_t regex_batch_raw(const char *who, const search_params_t *P, const 
     DeviceGuard guard;
     std::vector<uint64_t> off(n_texts, 0);
     HostScan hs;
-    const int rc = regex_batch_scan(plan, texts, lens, live, mode, long_lines, who, &off, &hs);
+    const int rc = regex_batch_scan(plan, texts, lens, live, (RegexMode)mode, long_lines, who, &off, &hs);
     if (rc != 0) return rc;
     for (size_t i = 0; i < live.size(); i++)
     {
         if (offsets) offsets[live[i]] = off[live[i]];
-        if (text_lines && mode == 1) text_lines[live[i]] = hs.text_lines[i];
+        if (text_lines && mode == RX_COUNT) text_lines[live[i]] = hs.text_lines[i];
     }
     if (hs.nkeys && cap) memcpy(keys, hs.keys, std::min<uint64_t>(hs.nkeys, cap) * sizeof(uint64_t));
     return (int64_t)hs.nkeys;
@@ -1939,8 +1900,7 @@ search_func_t krep_b200_select_search_algorithm(const search_params_t *P)
         // the regex goes to the GPU line filter when its compiler accepts the pattern; a refused one stays with the
         // host's regex_search
         std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-        std::string why;
-        return cached_regex_plan(P, &why) ? krep_b200_regex_search : NULL;
+        return regex_plan_of(P) ? krep_b200_regex_search : NULL;
     }
     if (P->num_patterns > 1) return krep_b200_aho_corasick_search;
     if (!g_algo_override.empty() && g_algo_override != "auto")
@@ -2118,8 +2078,7 @@ int krep_b200_count_lines_shard(const krep_b200_plan_t *plan_, const search_para
         return -3;
     }
     DeviceGuard guard;
-    cudaPointerAttributes a;
-    DevCtx *C = (cudaPointerGetAttributes(&a, shard->d_text) == cudaSuccess && a.type == cudaMemoryTypeDevice) ? ctx_get(a.device) : ctx_primary();
+    DevCtx *C = ctx_of_pointer(shard->d_text);
     if (!C) return -1;
     cudaStream_t st = stream ? (cudaStream_t)stream : C->scan_stream;
     reset_kernel_ms();
@@ -2173,9 +2132,7 @@ uint64_t krep_b200_search_shards(const krep_b200_plan_t *plan_, const search_par
     uint64_t text_len = 0;
     for (uint32_t i = 0; i < n_shards; i++)
     {
-        cudaPointerAttributes a;
-        ctx[i] = (cudaPointerGetAttributes(&a, shards[i].d_text) == cudaSuccess && a.type == cudaMemoryTypeDevice) ? ctx_get(a.device)
-                                                                                                                    : ctx_primary();
+        ctx[i] = ctx_of_pointer(shards[i].d_text);
         if (!ctx[i]) return 0;
         text_len = std::max<uint64_t>(text_len, shards[i].global_offset + shards[i].avail_len);
     }
@@ -2398,9 +2355,7 @@ int krep_b200_regex_export_shard(const krep_b200_plan_t *plan_, const search_par
 uint64_t krep_b200_regex_resolve(const search_params_t *P, const void *const *rows, uint32_t n_rows, match_result_t *result)
 {
     clear_error();
-    if (!P) return 0;
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    if (!P || regex_returns_early(P)) return 0;
     int err = 0;
     const uint64_t ret = regex_resolve_rows(P, rows, n_rows, result, &err);
     return err ? 0 : ret;
@@ -2418,8 +2373,7 @@ int64_t krep_b200_regex_filter_host(const search_params_t *P, const char *text, 
                                     int *widened)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl) return -1;
     std::vector<uint64_t> v;
     regex_lines_host(*pl->rx, text, text ? n : 0, &v);
@@ -2432,8 +2386,7 @@ int64_t krep_b200_regex_filter_host(const search_params_t *P, const char *text, 
 int krep_b200_regex_count_mode(const search_params_t *P)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl) return -1;
     return regex_count_fused(P, pl) ? 1 : 0;
 }
@@ -2441,24 +2394,22 @@ int krep_b200_regex_count_mode(const search_params_t *P)
 int64_t krep_b200_regex_count_host(const search_params_t *P, const char *text, size_t n, uint64_t reach)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl || !regex_count_exact(P, pl)) return -1;
-    if (P->max_count == 0 || !P->compiled_regex) return 0; // run_regex's early returns
-    if (n == 0) return (int64_t)replay_regex(P, Replay{nullptr, 0, text, 0, 0}, nullptr);
+    if (regex_returns_early(P)) return 0;
+    if (n == 0) return (int64_t)regex_empty_text(P, nullptr);
     if (!text) return 0;
     std::vector<uint64_t> keys;
     const uint64_t device_lines = regex_count_lines_host(*pl->rx, text, n, reach, &keys);
     for (uint64_t &k : keys) k <<= LIT_TAG_BITS;
-    return (int64_t)regex_count_total(P, device_lines, Replay{keys.data(), keys.size(), text, n, 0});
+    return (int64_t)regex_answer(P, RX_COUNT, device_lines, Replay{keys.data(), keys.size(), text, n, 0}, nullptr);
 }
 
 // ---- test hooks: split plans (DESIGN §12.7) ----
 int krep_b200_regex_automata(const search_params_t *P)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl) return -1;
     return pl->rx->groups.empty() ? 1 : (int)pl->rx->groups.size();
 }
@@ -2484,18 +2435,20 @@ int64_t krep_b200_regex_plan_host(const krep_b200_plan_t *plan_, int mode, const
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
     clear_error();
     const Plan *plan = reinterpret_cast<const Plan *>(plan_);
-    if (!plan || !plan->is_regex || (!text && n) || (cap && !keys) || mode < 0 || mode > 2 ||
-        (mode == 1 && !plan->rx->count_exact) || (mode == 2 && !plan->rx->offsets_exact))
+    if (!plan || !plan->is_regex || (!text && n) || (cap && !keys) || !regex_mode_available(*plan->rx, mode))
     {
         set_error(-3, "krep_b200_regex_plan_host: bad argument, or mode %d is not available for this plan", mode);
         return -3;
     }
     std::vector<uint64_t> v;
     uint64_t lines = 0;
-    if (mode == 0) regex_lines_host(*plan->rx, text, n, &v);
-    else if (mode == 1) lines = regex_count_lines_host(*plan->rx, text, n, reach, &v);
-    else regex_matches_host(*plan->rx, text, n, reach, &v);
-    if (mode != 2)
+    switch (mode)
+    {
+    case RX_FILTER: regex_lines_host(*plan->rx, text, n, &v); break;
+    case RX_COUNT: lines = regex_count_lines_host(*plan->rx, text, n, reach, &v); break;
+    default: regex_matches_host(*plan->rx, text, n, reach, &v);
+    }
+    if (mode != RX_OFFSETS)
         for (uint64_t &k : v) k <<= LIT_TAG_BITS;
     for (size_t i = 0; i < v.size() && i < cap; i++) keys[i] = v[i];
     if (device_lines) *device_lines = lines;
@@ -2506,8 +2459,7 @@ int64_t krep_b200_regex_plan_host(const krep_b200_plan_t *plan_, int mode, const
 int krep_b200_regex_match_mode(const search_params_t *P)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl) return -1;
     return regex_matches_device(P, pl) ? 1 : 0;
 }
@@ -2515,15 +2467,14 @@ int krep_b200_regex_match_mode(const search_params_t *P)
 int64_t krep_b200_regex_matches_host(const search_params_t *P, const char *text, size_t n, uint64_t reach, match_result_t *res)
 {
     std::lock_guard<std::recursive_mutex> lk(engine_mutex());
-    std::string why;
-    Plan *pl = P ? cached_regex_plan(P, &why) : nullptr;
+    Plan *pl = regex_plan_of(P);
     if (!pl || !regex_matches_exact(P, pl)) return -1;
-    if (P->max_count == 0 || !P->compiled_regex) return 0; // run_regex's early returns
-    if (n == 0) return (int64_t)replay_regex(P, Replay{nullptr, 0, text, 0, 0}, res);
+    if (regex_returns_early(P)) return 0;
+    if (n == 0) return (int64_t)regex_empty_text(P, res);
     if (!text) return 0;
     std::vector<uint64_t> keys;
     regex_matches_host(*pl->rx, text, n, reach, &keys);
-    return (int64_t)replay_regex_matches(P, Replay{keys.data(), keys.size(), text, n, 0}, res);
+    return (int64_t)regex_answer(P, RX_OFFSETS, 0, Replay{keys.data(), keys.size(), text, n, 0}, res);
 }
 
 } // extern "C"

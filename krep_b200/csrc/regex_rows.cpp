@@ -32,7 +32,7 @@ struct RowView
 bool view_row(const void *row, uint64_t mode, RowView *v)
 {
     const RegexRowHeader *h = (const RegexRowHeader *)row;
-    if (!h || h->magic != REGEX_ROW_MAGIC || h->mode > 2 || h->mode != mode) return false;
+    if (!h || h->magic != REGEX_ROW_MAGIC || h->mode > RX_OFFSETS || h->mode != mode) return false;
     const uint8_t *b = (const uint8_t *)h;
     v->h = h;
     v->keys = (const uint64_t *)(b + sizeof(RegexRowHeader));
@@ -62,11 +62,10 @@ uint64_t resolve_views(const search_params_t *P, const std::vector<RowView> &v, 
                        bool at_end, match_result_t *res, int *err)
 {
     const uint32_t n_rows = (uint32_t)v.size();
-    const uint64_t mode = v[0].h->mode;
     if (n == 0)
     {
         *err = 0;
-        return at_end ? replay_regex(P, Replay{nullptr, 0, nullptr, 0, 0}, res) : 0; // krep.c:1403-1416
+        return at_end ? regex_empty_text(P, res) : 0;
     }
 
     // windows: the segments in text order, a segment cut at its shard's readable end completed from the heads after it
@@ -124,14 +123,7 @@ uint64_t resolve_views(const search_params_t *P, const std::vector<RowView> &v, 
         }
     }
     *err = 0;
-    uint64_t ret;
-    if (mode == 2) ret = replay_regex_matches_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last_byte, res);
-    else if (mode == 1)
-        ret = std::min<uint64_t>(device_lines + replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n,
-                                                                     last_byte, at_end, nullptr),
-                                 P->max_count);
-    else ret = replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last_byte, at_end, res);
-    return ret;
+    return regex_answer_windows(P, (RegexMode)v[0].h->mode, device_lines, keys, win, n, last_byte, at_end, res);
 }
 } // namespace
 
@@ -183,8 +175,9 @@ int regex_resolve_batch(const search_params_t *P, const void *row, size_t n_text
         set_error(-3, "regex batch: not a regex row");
         return -3;
     }
-    const uint64_t mode = v.h->mode, nkeys = v.h->nkeys, nseg = v.h->nseg;
-    const int shift = mode == 2 ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+    const RegexMode mode = (RegexMode)v.h->mode;
+    const uint64_t nkeys = v.h->nkeys, nseg = v.h->nseg;
+    const int shift = regex_key_shift(mode);
     std::vector<const char *> bytes(nseg);
     const char *p = v.bytes;
     for (uint64_t s = 0; s < nseg; s++)
@@ -213,14 +206,8 @@ int regex_resolve_batch(const search_params_t *P, const void *row, size_t n_text
             const uint64_t sb = std::max<uint64_t>(v.segs[s].start, b), se = std::min<uint64_t>(v.segs[s].start + (v.segs[s].len_cont >> 1), e);
             if (se > sb) win.push_back(RegexWindow{(size_t)(sb - b), bytes[s] + (sb - v.segs[s].start), (size_t)(se - sb)});
         }
-        match_result_t *r = res ? res[i] : nullptr;
-        const size_t n = len[i];
-        if (mode == 2) counts[i] = replay_regex_matches_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last[i], r);
-        else if (mode == 1)
-            counts[i] = std::min<uint64_t>(text_lines[i] + replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n,
-                                                                                last[i], true, nullptr),
-                                           P->max_count);
-        else counts[i] = replay_regex_windows(P, keys.data(), keys.size(), win.data(), win.size(), n, last[i], true, r);
+        counts[i] = regex_answer_windows(P, mode, mode == RX_COUNT ? text_lines[i] : 0, keys, win, len[i], last[i], true,
+                                         res ? res[i] : nullptr);
     }
     return 0;
 }
@@ -234,8 +221,7 @@ uint64_t krep_b200_regex_resolve_part(const search_params_t *P, const void *cons
 {
     clear_error();
     if (!P) return 0;
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0; // krep.c:1395
-    if (!P->compiled_regex) return 0;                                              // krep.c:1399
+    if (regex_returns_early(P)) return 0;
     if (!rows || n_own == 0 || n_own > n_rows || (text_len && (last_byte < 0 || last_byte > 255)))
     {
         set_error(-3, "krep_b200_regex_resolve_part: needs 1 <= n_own <= n_rows rows, and the last byte of a non-empty text");
@@ -304,7 +290,7 @@ int krep_b200_regex_tiling(const void *headers, uint32_t n, krep_b200_regex_tili
     for (uint32_t i = 0; i < n; i++)
     {
         const RegexRowHeader &h = *hdr(i);
-        const bool row_ok = h.magic == REGEX_ROW_MAGIC && h.mode <= 2 && h.mode == hdr(0)->mode;
+        const bool row_ok = h.magic == REGEX_ROW_MAGIC && h.mode <= RX_OFFSETS && h.mode == hdr(0)->mode;
         const bool first_ok = i > 0 || (h.own_begin == 0 && !(h.flags & ROW_HEAD)); // the text starts at a line start
         const bool abut = i == 0 || hdr(i - 1)->own_end == h.own_begin;
         // a shard ends the text when it owns up to its end; only empty shards may follow it (shard_bounds gives trailing

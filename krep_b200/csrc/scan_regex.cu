@@ -73,13 +73,6 @@ __device__ __forceinline__ void emit_key(const RegexLaunch &a, uint64_t key)
     if (base < a.cap) a.out[base] = key;
 }
 
-enum RxMode : int
-{
-    RX_FILTER = 0, // one key per flagged line
-    RX_COUNT = 1,  // fused -c: lines decided MATCHED are counted, uncertain lines leave keys
-    RX_MATCH = 2,  // offsets: one key per match of a line decided MATCHED, uncertain lines leave keys
-};
-
 // Batch count mode: adds the thread's lines of text t to that text's counter.
 template <int MODE>
 __device__ __forceinline__ void add_text_lines(const RegexLaunch &a, uint32_t t, uint32_t &counted)
@@ -96,7 +89,7 @@ __device__ __forceinline__ void add_text_lines(const RegexLaunch &a, uint32_t t,
 // (RegexDfa::count_exact).  A line the walk decides (MATCHED or DEAD, or its '\n' read through the '\n' column) is
 // settled on the device, and a MATCHED one is counted; only the uncertain lines leave as keys: a line whose '\n' lies
 // beyond the walk's limit, and the line that holds the text's last byte (decided or not, so that both end-of-text
-// quirks of the reference stay with glibc: DESIGN §12.1).  RX_MATCH (RegexDfa::offsets_exact): the same uncertain
+// quirks of the reference stay with glibc: DESIGN §12.1).  RX_OFFSETS (RegexDfa::offsets_exact): the same uncertain
 // lines leave keys (REGEX_MATCH_SHIFT layout); a line decided MATCHED is enumerated with the anchored match automaton
 // (DESIGN §12.2) within a step budget, and a line over its budget leaves an uncertain key as well.
 // BATCH (krep_b200_regex_search_batch, DESIGN §12.5): the text is many texts packed with '\n' gaps.  Three rules differ:
@@ -116,8 +109,8 @@ __global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ?
     uint16_t *s_tab = reinterpret_cast<uint16_t *>(s_raw);
     const uint32_t tab_words = (a.ntrans + 7) & ~7u; // the class map follows the table, 16-byte aligned
     // match mode: the match table follows the class map (split plans: the match tables follow all line tables)
-    const uint32_t nvec = G > 1 ? (MODE == RX_MATCH ? a.image_words : a.line_words) / 8
-                                : (tab_words * 2 + 256 + (MODE == RX_MATCH ? regex_tab_words(a.nmtrans) * 2 : 0u)) / 16;
+    const uint32_t nvec = G > 1 ? (MODE == RX_OFFSETS ? a.image_words : a.line_words) / 8
+                                : (tab_words * 2 + 256 + (MODE == RX_OFFSETS ? regex_tab_words(a.nmtrans) * 2 : 0u)) / 16;
     const uint4 *src = reinterpret_cast<const uint4 *>(a.trans);
     for (uint32_t i = threadIdx.x; i < nvec; i += blockDim.x) s_raw[i] = src[i];
     __syncthreads();
@@ -232,7 +225,7 @@ __global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ?
                 }
                 else flag = true;                                                        // line not seen to its end: unverified
             }
-            if constexpr (MODE == RX_MATCH && G > 1)
+            if constexpr (MODE == RX_OFFSETS && G > 1)
             {
                 if (!flag && row == 0)
                 {
@@ -272,7 +265,7 @@ __global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ?
                     flag = steps > budget; // over budget: the whole line goes to regexec
                 }
             }
-            else if constexpr (MODE == RX_MATCH)
+            else if constexpr (MODE == RX_OFFSETS)
             {
                 if (!flag && row == 0)
                 {
@@ -312,7 +305,7 @@ __global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ?
                 unsigned long long base = 0;
                 if (g.thread_rank() == 0) base = atomicAdd(a.counter, (unsigned long long)g.size());
                 base = g.shfl(base, 0) + g.thread_rank();
-                if (base < a.cap) a.out[base] = (a.global_offset + p) << (MODE == RX_MATCH ? REGEX_MATCH_SHIFT : LIT_TAG_BITS);
+                if (base < a.cap) a.out[base] = (a.global_offset + p) << (MODE == RX_OFFSETS ? REGEX_MATCH_SHIFT : LIT_TAG_BITS);
             }
             if constexpr (MODE == RX_FILTER)
                 if (row <= dead) q = next_newline(W, q, limit);
@@ -335,7 +328,7 @@ __global__ void __launch_bounds__(G == 1 ? RX_THREADS : RX_SET_THREADS, G == 1 ?
 template <int MODE, bool BATCH>
 static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
-    const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256 + (MODE == RX_MATCH ? (size_t)regex_tab_words(a.nmtrans) * 2 : 0);
+    const size_t smem = (size_t)((a.ntrans + 7) & ~7u) * 2 + 256 + (MODE == RX_OFFSETS ? (size_t)regex_tab_words(a.nmtrans) * 2 : 0);
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_regex_lines<MODE, BATCH, 1>, RX_THREADS, smem) != cudaSuccess || per_sm < 1)
     {
@@ -347,7 +340,7 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
     const uint64_t resident = (uint64_t)sm_count * per_sm;
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
     trace("regex%s%s: %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", BATCH ? " batch" : "",
-          MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", grid, RX_THREADS, per_sm, smem);
+          MODE == RX_COUNT ? " count" : MODE == RX_OFFSETS ? " match" : "", grid, RX_THREADS, per_sm, smem);
     k_regex_lines<MODE, BATCH, 1><<<grid, RX_THREADS, smem, s>>>(a);
     count_launch();
 }
@@ -355,7 +348,7 @@ static void launch_regex_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 template <int MODE, bool BATCH, int G>
 static int launch_regex_sets_t(const RegexLaunch &a, int sm_count, cudaStream_t s)
 {
-    const size_t smem = (size_t)(MODE == RX_MATCH ? a.image_words : a.line_words) * 2;
+    const size_t smem = (size_t)(MODE == RX_OFFSETS ? a.image_words : a.line_words) * 2;
     // above the default 48 KiB a kernel must opt in, once per device (the attribute belongs to the current device)
     static std::atomic<bool> opted_in[MAX_DEV];
     int dev = 0;
@@ -387,7 +380,7 @@ static int launch_regex_sets_t(const RegexLaunch &a, int sm_count, cudaStream_t 
     const uint64_t resident = (uint64_t)sm_count * per_sm;
     const unsigned grid = (unsigned)(blocks_needed == 0 ? 1 : blocks_needed < resident ? blocks_needed : resident);
     trace("regex sets%s%s: %u automata, %u CTAs x %d threads (%d per SM), %zu bytes of shared memory", BATCH ? " batch" : "",
-          MODE == RX_COUNT ? " count" : MODE == RX_MATCH ? " match" : "", a.ngroups, grid, RX_SET_THREADS, per_sm, smem);
+          MODE == RX_COUNT ? " count" : MODE == RX_OFFSETS ? " match" : "", a.ngroups, grid, RX_SET_THREADS, per_sm, smem);
     k_regex_lines<MODE, BATCH, G><<<grid, RX_SET_THREADS, smem, s>>>(a);
     count_launch();
     return 0;
@@ -408,21 +401,21 @@ int launch_regex(const RegexLaunch &a, int sm_count, cudaStream_t s)
         if (a.text_end)
         {
             if (a.text_lines) return launch_regex_sets<RX_COUNT, true>(a, sm_count, s);
-            if (a.matches) return launch_regex_sets<RX_MATCH, true>(a, sm_count, s);
+            if (a.matches) return launch_regex_sets<RX_OFFSETS, true>(a, sm_count, s);
             return launch_regex_sets<RX_FILTER, true>(a, sm_count, s);
         }
         if (a.line_count) return launch_regex_sets<RX_COUNT, false>(a, sm_count, s);
-        if (a.matches) return launch_regex_sets<RX_MATCH, false>(a, sm_count, s);
+        if (a.matches) return launch_regex_sets<RX_OFFSETS, false>(a, sm_count, s);
         return launch_regex_sets<RX_FILTER, false>(a, sm_count, s);
     }
     if (a.text_end)
     {
         if (a.text_lines) launch_regex_t<RX_COUNT, true>(a, sm_count, s);
-        else if (a.matches) launch_regex_t<RX_MATCH, true>(a, sm_count, s);
+        else if (a.matches) launch_regex_t<RX_OFFSETS, true>(a, sm_count, s);
         else launch_regex_t<RX_FILTER, true>(a, sm_count, s);
     }
     else if (a.line_count) launch_regex_t<RX_COUNT, false>(a, sm_count, s);
-    else if (a.matches) launch_regex_t<RX_MATCH, false>(a, sm_count, s);
+    else if (a.matches) launch_regex_t<RX_OFFSETS, false>(a, sm_count, s);
     else launch_regex_t<RX_FILTER, false>(a, sm_count, s);
     return 0;
 }

@@ -317,12 +317,12 @@ int regex_pack_row(DevCtx &E, const krep_b200_shard_t *sh, int mode, const uint6
     g.G = sh->global_offset;
     g.prev_byte = sh->prev_byte;
     g.next_byte = sh->next_byte;
-    g.shift = mode == 2 ? REGEX_MATCH_SHIFT : LIT_TAG_BITS;
+    g.shift = regex_key_shift((RegexMode)mode);
     const unsigned grid_n = (unsigned)std::min<uint64_t>((n + PK_THREADS - 1) / PK_THREADS, (uint64_t)E.sm_count * 16);
     CKP(cudaEventRecord(B.ev0, st));
     CKP(cudaMemsetAsync(B.meta, 0, PM_WORDS * 8, st));
     // the lines glibc must see, in key order (NumSelected lands in meta[PM_NSEL])
-    const IsLine pred{mode == 2 ? 1 : 0};
+    const IsLine pred{mode == RX_OFFSETS};
     size_t need = 0, need2 = 0, need3 = 0;
     CKP(cub::DeviceSelect::If(nullptr, need, d_keys, B.sel, B.meta + PM_NSEL, (int64_t)nkeys, pred, st));
     CKP(cub::DeviceScan::ExclusiveSum(nullptr, need2, B.flag, B.segid, (int64_t)n, st));

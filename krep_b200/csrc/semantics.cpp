@@ -567,6 +567,19 @@ uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *re
 }
 
 // ---- regex_search (krep.c:1389-1579) over the lines the device flagged ----------------------------------------------
+bool regex_returns_early(const search_params_t *P)
+{
+    return (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) || !P->compiled_regex;
+}
+
+uint64_t regex_empty_text(const search_params_t *P, match_result_t *res)
+{
+    regmatch_t m;
+    if (regexec((const regex_t *)P->compiled_regex, "", 1, &m, 0) != 0) return 0;
+    if (!P->count_lines_mode && P->track_positions && res) result_push(res, 0, 0);
+    return 1;
+}
+
 // Under REG_NEWLINE no match contains a '\n' (regex_dfa.cpp refuses character sets that hold one), so the reference loop
 // is unchanged if (1) the cursor skips every line the filter did not flag — glibc finds no match starting there, from
 // the line start or from any position inside it — and (2) each regexec call is clipped to the run of consecutive
@@ -588,22 +601,11 @@ uint64_t replay_ac(const search_params_t *P, const Replay &r, match_result_t *re
 #endif
 uint64_t replay_regex(const search_params_t *P, const Replay &r, match_result_t *res)
 {
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0;
-    if (!P->compiled_regex) return 0;
+    if (regex_returns_early(P)) return 0;
     const regex_t *regex = (const regex_t *)P->compiled_regex;
     const char *t = r.text;
     const size_t n = r.text_len;
-    if (n == 0)
-    {
-        regmatch_t m;
-        if (regexec(regex, "", 1, &m, 0) == 0)
-        {
-            if (P->count_lines_mode) return 1;
-            if (P->track_positions && res) result_push(res, 0, 0);
-            return 1;
-        }
-        return 0;
-    }
+    if (n == 0) return regex_empty_text(P, res);
     // krep.c:1422 passes compilation flags as execution flags: REG_NEWLINE has the value of REG_STARTEND and REG_ICASE
     // the value of REG_NOTEOL.  Passed on exactly as the reference does.
     const int base_eflags = REG_STARTEND | REG_NEWLINE | (P->case_sensitive ? 0 : REG_ICASE);
@@ -792,7 +794,7 @@ uint64_t replay_regex_matches(const search_params_t *P, const Replay &r, match_r
 uint64_t replay_regex_windows(const search_params_t *P, const uint64_t *keys, size_t nkeys, const RegexWindow *w, size_t nw,
                               size_t n, int last_byte, bool at_end, match_result_t *res)
 {
-    if (P->max_count == 0 && (P->count_lines_mode || P->track_positions)) return 0;
+    if (regex_returns_early(P)) return 0;
     const size_t max_count = P->max_count;
     uint64_t count = 0;
     size_t j = 0, covered = 0; // covered: end of the last window replayed
@@ -884,6 +886,42 @@ uint64_t replay_regex_matches_windows(const search_params_t *P, const uint64_t *
         count += replay_regex_windows(&sub, lines.data(), lines.size(), w + wi, nw - wi, n, last_byte, false, res);
     }
     return count;
+}
+
+// The filter's keys are the flagged lines replay_regex confirms; the offsets mode's are match and uncertain-line keys
+// (replay_regex_matches, DESIGN §12.2).  The fused -c answers  min(lines the device decided MATCHED + replay_regex over
+// the uncertain lines, max_count).  Why this is the reference's count: without -w and -o the loop of krep.c:1389-1579
+// calls regexec only at line starts (after a counted line the cursor jumps to the next line start; with no match left
+// the loop ends) and never with REG_NOTBOL, and under REG_NEWLINE no match contains a '\n'.  So a line is counted
+// exactly when glibc finds a match in it from its start, each line independently of the others — which the automaton of
+// a count_exact plan decides — and the -m limit only caps the total.  Two answers depend on the end of the text rather
+// than on one line: '$' cannot match at the end of the text under -i (REG_ICASE passed as an execution flag is
+// REG_NOTEOL), and a text that ends in '\n' holds an empty string at n that is counted when the last line was not and
+// the regex matches there.  The line holding the text's last byte is always among the uncertain keys, so both are
+// decided inside glibc's last run, as in the reference; skipping the lines counted on the device changes nothing for the
+// runs in between, since each run starts at a line start.
+uint64_t regex_answer(const search_params_t *P, RegexMode mode, uint64_t device_lines, const Replay &r, match_result_t *res)
+{
+    switch (mode)
+    {
+    case RX_COUNT: return std::min<uint64_t>(device_lines + replay_regex(P, r, nullptr), P->max_count);
+    case RX_OFFSETS: return replay_regex_matches(P, r, res);
+    default: return replay_regex(P, r, res);
+    }
+}
+
+uint64_t regex_answer_windows(const search_params_t *P, RegexMode mode, uint64_t device_lines, const std::vector<uint64_t> &keys,
+                              const std::vector<RegexWindow> &w, size_t n, int last_byte, bool at_end, match_result_t *res)
+{
+    switch (mode)
+    {
+    case RX_COUNT:
+        return std::min<uint64_t>(
+            device_lines + replay_regex_windows(P, keys.data(), keys.size(), w.data(), w.size(), n, last_byte, at_end, nullptr),
+            P->max_count);
+    case RX_OFFSETS: return replay_regex_matches_windows(P, keys.data(), keys.size(), w.data(), w.size(), n, last_byte, res);
+    default: return replay_regex_windows(P, keys.data(), keys.size(), w.data(), w.size(), n, last_byte, at_end, res);
+    }
 }
 
 } // namespace kb

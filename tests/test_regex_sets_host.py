@@ -422,3 +422,32 @@ def test_split_plan_hook_arguments():
         assert sp.host(0, b"ab\nx\ncd\n") == ([0 << 3, 5 << 3], 0)
     finally:
         sp.close()
+
+
+@pytest.mark.parametrize("pats,cap,admits", [
+    (["the[a-z]*"], 4096, {0, 1, 2}),
+    (["\\bab", "cd"], 4096, {0}),                                            # widened: the filter only
+    (lower_words(random.Random(1), 60), 4096, {0, 1}),                       # no room for the match table
+    (lower_words(random.Random(7), 200) + ["the[a-z]*"], 4096, {0, 1, 2}),  # split
+    (alnum_words(random.Random(7), 200), 4096, {0, 1}),                      # split, line tables only
+    (lower_words(random.Random(3), 80) + ["\\bab"], 4096, {0}),              # split, widened
+    (["abc", "xyz", "q[0-9]+"], 6, {0, 1, 2}),                               # split by the lowered cap
+    (["ab\\b", "cd", "efg"], 6, {0}),
+])
+def test_plan_host_refuses_modes_the_plan_lacks(pats, cap, admits):
+    # modes outside 0..2, and the count / match modes of plans not exact for them, are refused as a bad argument
+    L = lib.load()
+    sp = SplitPlan(_params(pats), cap)
+    try:
+        assert sp.h, pats
+        keys = (C.c_uint64 * 8)()
+        dl = C.c_uint64(0)
+        for mode in (-1, 0, 1, 2, 3):
+            k = L.krep_b200_regex_plan_host(sp.h, mode, b"abc the\nxyz q1\n", 15, UNBOUNDED, keys, 8, C.byref(dl))
+            err = L.krep_b200_last_error()
+            if mode in admits:
+                assert k >= 0 and err == 0, (mode, k, err)
+            else:
+                assert k == -3 and err == -3, (mode, k, err)
+    finally:
+        sp.close()
